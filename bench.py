@@ -8,7 +8,7 @@ eval-mode BatchNorm, forward only, on a batch of synthetic dental-arch clouds of
     FPS 24000->1024  ->  ball query (r=0.1, K=32)  ->  fused gather+MLP(9->32->32->64)+max.
 metric = sampled points per second = clouds * 1024 / time, whole job (all ranks).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--clouds B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--clouds B] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 * ``value``: the PUBLIC module call ``sa(xyz, feats)`` with inputs resident in HBM, CUDA-event timed, max over ranks.
@@ -16,16 +16,20 @@ metric = sampled points per second = clouds * 1024 / time, whole job (all ranks)
 * ``e2e``: the same step through ``HostPipeline(sa)`` with HOST (pinned) inputs: H2D copy of the (B,6,N) feature
   tensor and D2H copy of both outputs inside the timed region.  Each rank binds itself and its pinned buffers to
   its GPU's NUMA node first (``numa``).
-* ``roofline``: the dominant kernel (FPS), real DRAM traffic / time against the measured HBM copy peak;
+* ``roofline``: the dominant kernel (FPS), compulsory DRAM bytes / time against the HBM peak;
   ``roofline_stages``: one entry per stage (FPS: HBM; ball query: fp32 issue; group-MLP: tensor pipe).
 * ``parity_ok``: cloud 0 of this rank against the CPU oracle (indices bitwise, features element-wise 1e-4).
 * ``ref_gpu``: the REFERENCE's own GPU path for the same step (verbatim FPS kernel from ``oracle/_ref`` + the reference's
   torch ball query / gather / Conv2d+BN+ReLU / max), timed with CUDA events on this GPU (rank 0, bounded batch).
-* ``latency_ms``: FPS latency at B in {1,16,148,1184} x M in {1024,4096} (``c1`` = BASELINE configs[0], 24000->4096 on
+* ``--dump-outputs DIR``: after the timed steps, rank 0 writes what the last timed ``sa(xyz, feats)`` returned as
+  ``DIR/new_xyz.npy`` and ``DIR/new_points.npy`` (float32) for a fixed, seeded sample of at most 64 of its clouds (sorted
+  cloud order; ``DIR/sample_clouds.npy`` holds their indices as float64).  Inputs are synthesised from fixed seeds, so two
+  builds run with the same arguments can be compared output for output.
+* ``latency_ms``: FPS latency at B in {1,16,132,1056} x M in {1024,4096} (``c1`` = BASELINE configs[0], 24000->4096 on
   one cloud, bit-exact against the reference kernel), ``knn``: the tgnet_fps kNN launch mix beside the reference kernel.
 * ``cpu_baseline`` / ``--impl reference``: the oracle's port of the reference's CPU-capable formulation of the same
   path (FPS loop + query_ball_point + grouped MLP, one cloud per host thread), bounded sample.
-Inputs are larger than L2 (B*24000*6*4 bytes = 682 MB at the default B = 1184); no explicit flush.
+Inputs are larger than L2 (B*24000*6*4 bytes = 608 MB at the default B = 1056); no explicit flush.
 """
 from __future__ import annotations
 
@@ -50,7 +54,7 @@ METRIC = "sampled-points/sec (FPS+ballq+group-MLP, 24k-pt cloud)"
 UNIT = "sampled points/s"
 WORKLOAD = "pointnet++ SA1 forward: FPS 24000->1024, ball query r=0.1 K=32, group-MLP 9->[32,32,64], eval BN"
 MLP_FLOP_PER_CLOUD = 2.0 * NPOINT * NSAMPLE * (9 * 32 + 32 * 32 + 32 * 64)      # SURVEY.md 8d: 0.220 GFLOP
-B200_FP32_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12                                  # CUDA-core FMA peak at max clock
+H100_FP32_TFLOPS = 67.0                                                            # H100 SXM data sheet, CUDA-core fp32, 700 W
 
 
 def host_cores() -> int:
@@ -75,14 +79,7 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1590.0}, "fallback"
-
-
-def ncu_constants():
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "ncu_constants.json")))
-    except Exception:
-        return {}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback"     # H100 SXM data sheet (dense)
 
 
 # ------------------------------------------------------------------------------------------ NUMA
@@ -256,6 +253,15 @@ def elementwise_rel(a: torch.Tensor, b: torch.Tensor, floor: float = 0.05) -> fl
     return float(((a - b).abs() / b.abs().clamp(min=floor * float(b.abs().max()) + 1e-300)).max())
 
 
+def dump_outputs(out_dir: str, B: int, outputs) -> None:
+    """The last timed step's (new_xyz, new_points) for a seeded sample of at most 64 clouds, float32 (<= 18 MB)."""
+    pick = torch.sort(torch.randperm(B, generator=torch.Generator().manual_seed(0))[:min(B, 64)]).values
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "sample_clouds.npy"), pick.numpy().astype(np.float64))
+    for name, t in zip(("new_xyz", "new_points"), outputs):
+        np.save(os.path.join(out_dir, f"{name}.npy"), t[pick.to(t.device)].float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------------------ main
 def main():
     ap = argparse.ArgumentParser()
@@ -263,19 +269,20 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--clouds", type=int, default=1184, help="clouds per GPU per step (8 per SM)")
+    ap.add_argument("--clouds", type=int, default=1056, help="clouds per GPU per step (8 per SM of an H100)")
     ap.add_argument("--cpu-clouds", type=int, default=0, help="clouds in the CPU sample (default: 2 per host core, at most 64)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the ref_gpu / latency / kNN / C1 legs (profiling runs)")
     ap.add_argument("--no-numa", action="store_true")
-    ap.add_argument("--e2e-chunk", type=int, default=148, help="clouds per pipelined chunk of the end-to-end measurement")
+    ap.add_argument("--e2e-chunk", type=int, default=132, help="clouds per pipelined chunk of the end-to-end measurement")
     ap.add_argument("--e2e-streams", type=int, default=2)
     ap.add_argument("--e2e-groups", default="1", help="chunks per compute group of the end-to-end pipeline")
     ap.add_argument("--e2e-sa-engine", type=int, default=None, help="group-MLP engine inside the end-to-end pipeline (5: half-size CTAs that co-reside with other chunks' kernels)")
     ap.add_argument("--e2e-fps-mode", type=int, default=None, help="FPS shape of every pipelined chunk (-14: 4 warps per cloud, -18: 8, -26: 16); default: by clouds in flight")
     ap.add_argument("--fps-mode", type=int, default=0, help="0 auto; 100*G+CS resident shape, -2 bucket, -(10+W) bucket with W warps per cloud (experiments)")
     ap.add_argument("--ball-path", type=int, default=0, help="0 auto, 4 index-order tile scan, 8 uniform grid (experiments)")
-    ap.add_argument("--sa-engine", type=int, default=0, help="0 auto, 1 fp32 CUDA cores, 2 tcgen05 (experiments)")
+    ap.add_argument("--sa-engine", type=int, default=0, help="0 auto, 1 fp32 CUDA cores, 2 3xTF32 tensor cores (experiments)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs (seeded sample of <= 64 clouds) as DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -370,9 +377,10 @@ def main():
         torch.cuda.synchronize()
         launches0 = L.launch_count()
         with ClockSampler(local) as clk:
+            last = None
             t_start.record()
             for s in range(args.steps):
-                sa(xyz, feats)
+                last = sa(xyz, feats)
             t_end.record()
             torch.cuda.synchronize()
         launches = L.launch_count() - launches0
@@ -388,6 +396,9 @@ def main():
     ball_ms = float(np.mean([e[1].elapsed_time(e[2]) for e in stage_events]))
     mlp_ms = float(np.mean([e[2].elapsed_time(e[3]) for e in stage_events]))
     value = world * B * NPOINT * args.steps / total_s
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, B, last)
+    del last
 
     # -------- end to end through the public API with host buffers -----------------------------------
     out_xyz_host = torch.empty((B, 3, NPOINT), dtype=torch.float32).pin_memory()
@@ -447,30 +458,23 @@ def main():
     if rank != 0:
         return
     peaks, peak_kind = measured_peaks()
-    ncu = ncu_constants()
     fps_alg_bytes = 20.0 * (NPOINT - 1) * N_POINTS * B            # per FPS launch (SURVEY.md 8d)
     fps_compulsory = (12.0 * N_POINTS + 4.0 * NPOINT) * B
-    fps_traffic = ncu.get("fps_dram_bytes_per_cloud", 0.0) * B or None
-    fps_dram_gbs = fps_traffic / (fps_ms * 1e-3) / 1e9 if fps_traffic else None
+    fps_dram_gbs = fps_compulsory / (fps_ms * 1e-3) / 1e9          # compulsory bytes: a lower bound on the DRAM traffic
     tensor_peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops"))
     mlp_tflops = MLP_FLOP_PER_CLOUD * B / (mlp_ms * 1e-3) / 1e12
     ball_tflops = 8.0 * NPOINT * N_POINTS * B / (ball_ms * 1e-3) / 1e12
     stages = [
         {"stage": "fps", "kernel": "fps_bucket_sort_kernel + fps_bucket_kernel", "bound": "hbm (latency of the per-sample dependent chain in practice)",
-         "ms": fps_ms, "compulsory_bytes": fps_compulsory, "traffic_bytes": fps_traffic, "traffic_over_compulsory": (fps_traffic / fps_compulsory) if fps_traffic else None,
-         "achieved": fps_dram_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": (fps_dram_gbs / peaks["hbm_gbs"]) if fps_dram_gbs else None,
+         "ms": fps_ms, "compulsory_bytes": fps_compulsory,
+         "achieved": fps_dram_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s (compulsory bytes / time)", "frac": fps_dram_gbs / peaks["hbm_gbs"],
          "algorithmic_bytes": fps_alg_bytes, "algorithmic_gbs": fps_alg_bytes / (fps_ms * 1e-3) / 1e9,
-         "traffic_source": ncu.get("fps_source"), "traffic_is": "constant from the committed ncu capture, scaled per cloud (not measured live)",
-         "note": "the exact bucket pruning skips ~97% of the brute-force point-updates, so algorithmic_gbs exceeds the HBM peak by construction; frac is real DRAM traffic / time / peak"},
+         "note": "the exact bucket pruning skips most brute-force point-updates, so algorithmic_gbs can exceed the HBM peak; frac is compulsory bytes / time / peak"},
         {"stage": "ball_query", "kernel": "ball_query_kernel (index-order tile scan at r=0.1)", "bound": "fp32 issue", "ms": ball_ms,
-         "achieved": ncu.get("ball_query_issue_active_pct"), "peak": 100.0, "unit": "% issue slots active (ncu, committed capture)",
-         "frac": (ncu.get("ball_query_issue_active_pct") or 0.0) / 100.0, "source": ncu.get("ball_query_source"),
-         "bruteforce_equivalent_tflops": ball_tflops, "fp32_peak_tflops": B200_FP32_TFLOPS,
+         "bruteforce_equivalent_tflops": ball_tflops, "fp32_peak_tflops": H100_FP32_TFLOPS,
          "note": "8*S*N FLOP per cloud / time exceeds the fp32 peak because the index-order scan stops after K hits; the bound that applies is instruction issue"},
-        {"stage": "group_mlp", "kernel": "sa_mlp_tc_kernel (tcgen05 3xTF32)", "bound": "tensor", "ms": mlp_ms, "achieved": mlp_tflops, "peak": tensor_peak,
-         "unit": "TFLOP/s useful (2*S*K*sum C_l*C_l+1)", "frac": mlp_tflops / tensor_peak, "peak_name": "bf16_tflops_sustained",
-         "executed_over_useful_mma": ncu.get("group_mlp_executed_over_useful_mma"), "tensor_pipe_pct": ncu.get("group_mlp_tensor_pipe_pct"),
-         "source": ncu.get("group_mlp_source")},
+        {"stage": "group_mlp", "kernel": "sa_mlp_tc_kernel (wgmma 3xTF32)", "bound": "tensor", "ms": mlp_ms, "achieved": mlp_tflops, "peak": tensor_peak,
+         "unit": "TFLOP/s useful (2*S*K*sum C_l*C_l+1)", "frac": mlp_tflops / tensor_peak, "peak_name": "bf16_tflops_sustained"},
     ]
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -479,8 +483,8 @@ def main():
         "stage_ms": {"fps": fps_ms, "ball_query": ball_ms, "group_mlp": mlp_ms},
         "roofline": {"kernel": "fps_bucket_kernel (+ its sort prologue; one event pair brackets both)", "bound": "hbm",
                      "achieved": fps_dram_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": stages[0]["frac"],
-                     "traffic": fps_traffic, "peak_kind": peak_kind, "compulsory_bytes": fps_compulsory,
-                     "note": "achieved = DRAM bytes of the launch pair (ncu, committed capture) / live CUDA-event time; the SURVEY 8d "
+                     "peak_kind": peak_kind, "compulsory_bytes": fps_compulsory,
+                     "note": "achieved = compulsory bytes of the launch pair / live CUDA-event time; the SURVEY 8d "
                              "algorithmic figure (20*(M-1)*N bytes per cloud) is in roofline_stages[0].algorithmic_gbs and is not a bandwidth"},
         "roofline_stages": stages,
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(host_feats.numel() * 4),
@@ -512,7 +516,7 @@ def extras(device) -> dict:
     import op_bench
     out = {}
     with torch.no_grad():
-        rows = op_bench.fps_latency_table(batches=(1, 16, 148, 1184), npoints=(1024, 4096), with_ref=op_bench.ref_available())
+        rows = op_bench.fps_latency_table(batches=(1, 16, 132, 1056), npoints=(1024, 4096), with_ref=op_bench.ref_available())
         out["latency_ms"] = {"fps": rows}
         c1 = next(r for r in rows if r["clouds"] == 1 and r["m"] == 4096)
         out["c1"] = dict(c1, config="BASELINE configs[0]: furthest_point_sample 24000->4096 on one cloud", **op_bench.c1_parity())

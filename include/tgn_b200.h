@@ -1,5 +1,5 @@
 /*
- * tgn_b200.h -- C ABI of libtgn_b200.so: the B200-native (sm_100a) replacement for the native
+ * tgn_b200.h -- C ABI of libtgn_b200.so: the H100-native (sm_90a) replacement for the native
  * layer of limhoyeon/ToothGroupNetwork's point-cloud operator hot path.
  *
  * Boundary being replaced (paths relative to /root/reference/external_libs/pointops/src):
@@ -196,8 +196,9 @@ int tgn_transpose_cn(int B, int C, int N, const float *in, float *out, void *str
  *   weights[l] (C_{l+1}, C_l) row-major DEVICE, biases[l] (C_{l+1}) DEVICE; the two pointer arrays are HOST arrays
  *   out: channel-first (B, out_c_total, S); this branch writes channels [out_c_offset, +C_last)
  *   engine: 0 = auto (2 when the shape fits it, else 3, else 1), 1 = fp32 CUDA-core kernel (exact FMA),
- *           2 = tcgen05 3xTF32 kernel (widths <= 64, ~2^-21), 3 = tcgen05 kernel for wide layers (first layer
- *           3xTF32, later layers as three bf16x2-split MMAs, ~1e-5; at least two layers, K in {16,32,64,128}). */
+ *           2 = tensor-core (wgmma) 3xTF32 kernel (widths <= 64, any K <= 128, ~2^-21), 3 = tensor-core kernel for wide layers
+ *           (first layer 3xTF32, later layers as three bf16x2-split MMAs, ~1e-5; at least two layers, K in {16,32,64,128}),
+ *           5 = engine 2 in half-size CTAs.  Any other value is refused (engine 4 was Blackwell-only and is gone). */
 int tgn_sa_group_mlp_max(int B, int N, int S, int K, int D, const float *xyz, const float *feats, const float *new_xyz,
                          const int *group_idx, int xyz_first, int n_layers, const int *channels,
                          const float *const *weights, const float *const *biases, float *out, int out_c_total,
@@ -212,7 +213,7 @@ int tgn_sa_group_mlp_max(int B, int N, int S, int K, int D, const float *xyz, co
  *      y[c, r] = sum_k W[c, k] * act(x)[r, k] + bias[c],   r in [0, rows)
  * where act() is the previous layer's BatchNorm + ReLU applied while the operand is built
  * (in_affine: 0 none, 1 from the fp64 batch sums `in_stats` = {sum[cin], sumsq[cin]} over `rows` rows,
- * 2 from running statistics).  tcgen05, operands split into three bf16 parts (six MMAs per K step, fp32-grade:
+ * 2 from running statistics).  wgmma, operands split into three bf16 parts (six MMAs per K step, fp32-grade:
  * batch-statistics BatchNorm amplifies rounding differences) or two (`precision` = 2: three MMAs, ~1e-5).
  * mode 0: the operand row r = (b, n), b = r / rows_per_batch, is read from up to two strided segments,
  *         x[k] = seg_ptr[i][b*seg_batch_stride[i] + n*seg_row_stride[i] + k'*seg_chan_stride[i]] (strides in floats);

@@ -14,7 +14,7 @@ Two layers:
 
 Parity pins: ``tests/golden/ref_torch_*.npz`` (reference python imported from /root/reference,
 generator ``tests/golden/make_ref_torch_golden.py``) and ``tests/golden/ref_cuda_*.npz``
-(reference CUDA kernels compiled verbatim, run on a B200, generator
+(reference CUDA kernels compiled verbatim, run on the GPU, generator
 ``tests/golden/make_ref_cuda_golden.py``).
 """
 from __future__ import annotations

@@ -7,8 +7,8 @@
  *
  * Parity status: the reference ships no tests and no golden vectors (SURVEY.md 4),
  * so this restatement is pinned against OUTPUTS OF THE REFERENCE ITSELF:
- *   - the reference CUDA kernels compiled verbatim for sm_100a (oracle/_ref,
- *     built by oracle/Makefile) run on a B200 -> tests/golden/ref_cuda_*.npz
+ *   - the reference CUDA kernels compiled verbatim for the GPU (oracle/_ref,
+ *     built by oracle/Makefile) run on the GPU -> tests/golden/ref_cuda_*.npz
  *     (generator: tests/golden/make_ref_cuda_golden.py);
  *   - the reference's pure-torch pointnet2_utils functions imported from
  *     /root/reference on CPU -> tests/golden/ref_torch_*.npz

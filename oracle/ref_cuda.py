@@ -3,7 +3,7 @@
 
 ``oracle/_ref/libpointops_ref.so`` is built by ``make -C oracle ref`` from the six unmodified
 ``external_libs/pointops/src/*/*_cuda_kernel.cu`` files where they lie under /root/reference
-(compiled for sm_100a; nothing is copied into this repo).  It exports the reference's
+(compiled for sm_90a; nothing is copied into this repo).  It exports the reference's
 ``extern "C" *_launcher`` entry points, which take raw device pointers and launch on the legacy
 default stream -- so every wrapper below synchronises before and after.
 """

@@ -1,12 +1,12 @@
-"""Why does a 148-cloud chunk take 4.5 ms inside the host pipeline?  Times the module forward at B=148 alone, with a concurrent
-H2D copy stream, and stage by stage."""
+"""How long does one chunk of the host pipeline take?  Times the module forward on one 132-cloud chunk alone, with a
+concurrent H2D copy stream, and stage by stage."""
 import sys, torch
 sys.path.insert(0, ".")
 import bench
 from toothgroupnetwork_b200 import pointnet2_utils as pn2
-B = 148
+B = 132
 sa = bench.build_module("cuda")
-host = bench.make_clouds(0, 1184).pin_memory()
+host = bench.make_clouds(0, 1056).pin_memory()
 feats = host[:B].cuda()
 xyz = feats[:, :3].contiguous()
 ev = lambda: torch.cuda.Event(enable_timing=True)

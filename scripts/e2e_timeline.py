@@ -4,8 +4,8 @@ sys.path.insert(0, ".")
 from toothgroupnetwork_b200 import clouds, pointnet2_utils as pn2
 import bench
 
-B = int(sys.argv[1]) if len(sys.argv) > 1 else 1184
-chunk = int(sys.argv[2]) if len(sys.argv) > 2 else 148
+B = int(sys.argv[1]) if len(sys.argv) > 1 else 1056
+chunk = int(sys.argv[2]) if len(sys.argv) > 2 else 132
 ns = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 mode = sys.argv[4] if len(sys.argv) > 4 else "all"      # all | h2d | compute
 host = bench.make_clouds(0, B).pin_memory()

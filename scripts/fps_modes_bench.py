@@ -4,7 +4,7 @@ sys.path.insert(0, "."); sys.path.insert(0, "scripts")
 import op_bench
 from toothgroupnetwork_b200 import pointops
 rows = []
-for B in (1, 16, 148, 296, 592, 1184):
+for B in (1, 16, 132, 264, 528, 1056):
     feats = op_bench.arch_batch(B, 24000)
     xyz = feats[:, :3].permute(0, 2, 1).contiguous().view(-1, 3)
     off = (torch.arange(1, B + 1, dtype=torch.int32) * 24000).cuda()

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Operator-level timings on one B200: this library beside the REFERENCE's own GPU path
+"""Operator-level timings on one GPU: this library beside the REFERENCE's own GPU path
 (verbatim ``pointops`` kernels from ``oracle/_ref`` + the reference's torch ``pointnet2_utils.py``),
 CUDA events on the launching stream, warm-up, median of ``reps``  (BASELINE.md 3: C1(a)/C2 "GPU
 reference"; VERDICT r1 items 3, 5(ii), 7).
@@ -78,7 +78,7 @@ def c1_parity():
 
 
 # ------------------------------------------------------------------------------------------ FPS
-def fps_latency_table(batches=(1, 16, 148, 1184), npoints=(1024, 4096), N=24000, with_ref=True, ref_max_batch=148):
+def fps_latency_table(batches=(1, 16, 132, 1056), npoints=(1024, 4096), N=24000, with_ref=True, ref_max_batch=132):
     """ms per call of FPS N->M over a batch of B clouds: ours (auto shape) and the verbatim reference kernel."""
     from toothgroupnetwork_b200 import pointops
     rows = []
@@ -356,4 +356,4 @@ def tgnet_nograd_row(points=24000):
     a, b = outs["b200"].double(), outs["reference"].double()
     err = float(((a - b).abs() / b.abs().clamp(min=0.05 * float(b.abs().max()))).max())
     return {"points": points, "ms": ms, "speedup_vs_reference_ops": ms["reference"] / ms["b200"], "sem_1_elementwise_vs_reference": err,
-            "note": "train-mode BatchNorm amplifies fp32 rounding for both sides; profiles/r2_model_parity_tgnet_nograd.json holds the float64 verdict"}
+            "note": "train-mode BatchNorm amplifies fp32 rounding for both sides; scripts/model_parity.py --cases tgni gives the float64 verdict"}

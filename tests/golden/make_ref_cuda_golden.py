@@ -1,8 +1,8 @@
 """Generate tests/golden/ref_cuda_*.npz by running the REFERENCE'S OWN CUDA KERNELS (compiled
-verbatim for sm_100a into oracle/_ref/libpointops_ref.so by ``make -C oracle ref``) on a B200:
+verbatim for the GPU into oracle/_ref/libpointops_ref.so by ``make -C oracle ref``) on the GPU:
 
-    gpurun -- 'python tests/golden/make_ref_cuda_golden.py gpurun_out/golden'
-    cp gpurun_out/golden/ref_cuda_*.npz tests/golden/
+    python tests/golden/make_ref_cuda_golden.py OUT_DIR        # on a GPU, from the repository root
+    cp OUT_DIR/ref_cuda_*.npz tests/golden/
 
 Inputs are regenerated from seeds by the tests (toothgroupnetwork_b200.clouds), only the reference
 outputs are stored.  These fixtures pin the CPU oracle (tests/test_oracle_golden.py) against the

@@ -77,5 +77,8 @@ def test_dbscan_class_refuses_what_it_does_not_implement():
         clustering.DBSCAN(eps=0.1, min_samples=3, metric="manhattan")
     with pytest.raises(clustering.L.TgnError):
         clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 2), np.float32))
-    with pytest.raises(clustering.L.TgnError):                        # no CPU path: the product fails loudly without a GPU
-        clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 3), np.float32))
+    if torch.cuda.is_available():
+        assert clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 3), np.float32)).labels_.tolist() == [0, 0, 0, 0]
+    else:
+        with pytest.raises(clustering.L.TgnError):                    # no CPU path: the product fails loudly without a GPU
+            clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 3), np.float32))

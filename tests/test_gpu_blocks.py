@@ -1,4 +1,4 @@
-"""Fused PointTransformerLayer / TransitionDown forwards (csrc/pt_layer.cu, the tcgen05 layer chain) against the fixtures written by
+"""Fused PointTransformerLayer / TransitionDown forwards (csrc/pt_layer.cu, the tensor-core layer chain) against the fixtures written by
 the reference's own blocks.py (tests/golden/ref_torch_blocks.npz) and against the oracle's float64 evaluation.  No reference
 checkout is needed at run time; tests/test_gpu_reference_live.py holds the live comparisons."""
 import os

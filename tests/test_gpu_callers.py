@@ -151,7 +151,7 @@ def _params(convs, bns):
 
 
 def test_pointnetpp_msg_encoder_decoder_eval_matches_oracle():
-    """tsg_centroid_module-shaped U-Net at reduced size: 3 MSG set abstractions (fused tcgen05 /
+    """tsg_centroid_module-shaped U-Net at reduced size: 3 MSG set abstractions (fused tensor-core /
     fp32 engines, or the unfused CUDA path where widths exceed 128) + 3 feature propagations, eval
     BN; outputs within 1e-4 relative of the CPU oracle stack."""
     torch.manual_seed(3)

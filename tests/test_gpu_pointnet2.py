@@ -259,7 +259,7 @@ def test_set_abstraction_msg_eval_matches_reference_fixture(golden_dir, engine):
 @pytest.mark.parametrize("engine", [pn2.ENGINE_AUTO, pn2.ENGINE_TCW, pn2.ENGINE_FP32])
 def test_real_pointnet_pp_sa1_shape_matches_reference_fixture(golden_dir, engine):
     """The real pointnet_pp SA1 (pointnet_pp.py:13: two 9->128->128 branches, K = 32 / 64) against a fixture made
-    by the reference's own Python (tests/golden/make_ref_torch_msg128_golden.py).  AUTO takes the wide tcgen05 engine."""
+    by the reference's own Python (tests/golden/make_ref_torch_msg128_golden.py).  AUTO takes the wide tensor-core engine."""
     fix = load(golden_dir, "ref_torch_msg128.npz")
     feats = torch.from_numpy(fix["feats"]).cuda()
     msg = pn2.PointNetSetAbstractionMsg(128, [0.05, 0.1], [32, 64], 6, [[128, 128], [128, 128]]).cuda().eval()
@@ -312,15 +312,16 @@ SA_SHAPES = [
     # (N, S, r, K, D, widths, engine)        BASELINE C2(i) at full size first
     (24000, 1024, 0.1, 32, 6, [32, 32, 64], pn2.ENGINE_TC),
     (24000, 1024, 0.1, 32, 6, [32, 32, 64], pn2.ENGINE_FP32),
-    (24000, 1024, 0.1, 32, 6, [32, 32, 64], pn2.ENGINE_TC8),      # eight tile groups per SM, bf16x3 operands
-    (4096, 1024, 0.1, 16, 6, [32, 32, 64], pn2.ENGINE_TC8),       # two neighbourhoods per warp
-    (6000, 1001, 0.1, 32, 6, [32, 32, 64], pn2.ENGINE_TC8),       # S not a multiple of 4: partial tile, scalar output path
-    (3000, 300, 0.15, 16, 0, [16], pn2.ENGINE_TC8),               # xyz only, single layer
-    (5000, 512, 0.1, 32, 13, [20, 40, 24, 60], pn2.ENGINE_TC8),   # four layers, odd widths, full 16-channel input
+    (24000, 1024, 0.1, 32, 6, [32, 32, 64], pn2.ENGINE_TC_HALF),  # the tensor-core engine in half-size CTAs
+    (4096, 1024, 0.1, 16, 6, [32, 32, 64], pn2.ENGINE_TCW),       # eight neighbourhoods per tile on the wide engine
+    (6000, 1001, 0.1, 32, 6, [32, 32, 64], pn2.ENGINE_TC),        # S not a multiple of 4: partial last tile
+    (3000, 300, 0.15, 16, 0, [16], pn2.ENGINE_TC),                # xyz only, single layer
+    (5000, 512, 0.1, 32, 13, [20, 40, 24, 60], pn2.ENGINE_TC),    # four layers, odd widths, full 16-channel input
     (4096, 1024, 0.1, 16, 6, [32, 32, 64], pn2.ENGINE_TC),
     (16384, 700, 0.1, 64, 6, [32, 32, 64], pn2.ENGINE_TC),
     (3000, 200, 0.15, 24, 6, [20, 40], pn2.ENGINE_TC),          # K that does not divide 128, odd widths
     (3000, 200, 0.15, 24, 0, [16], pn2.ENGINE_TC),              # xyz only, single layer
+    (3000, 200, 0.15, 20, 6, [20, 40], pn2.ENGINE_TC),          # K not a multiple of 8: neighbourhoods split fragment blocks
     (3000, 200, 0.15, 24, 61, [64, 64, 128], pn2.ENGINE_FP32),   # tsg_centroid sa2-like width
     (2000, 50, 0.3, 200, 6, [32, 48], pn2.ENGINE_FP32),          # K > 128: chunked groups
 ]
@@ -352,7 +353,7 @@ def test_fused_sa_matches_oracle(N, S, r, K, D, widths, engine):
 
 
 WIDE_SHAPES = [
-    # (N, S, r, K, D, widths)   the wide tcgen05 engine (tf32 first layer, bf16x2-split later layers)
+    # (N, S, r, K, D, widths)   the wide tensor-core engine (tf32 first layer, bf16x2-split later layers)
     (24000, 1024, 0.05, 64, 6, [128, 128]),          # real pointnet_pp SA1 branch (pointnet_pp.py:13)
     (24000, 1024, 0.025, 32, 6, [128, 128]),
     (6000, 500, 0.1, 16, 6, [64, 64, 128]),          # three layers, partial last tile

@@ -51,7 +51,7 @@ def _pack(cl, ms):
 
 
 @pytest.mark.parametrize("name,build,ms", FPS_CASES, ids=[c[0] for c in FPS_CASES])
-@pytest.mark.parametrize("mode", [0, 1, 2, 4, 8, 201, 202, 204, 208, -1, -2, -3, -42, -44, -48, -56, -72, -84, -88, -96, -112])   # 100*G + CS; -(40 + W): single-barrier bucket schedule; -(80 + W): + register-resident tables
+@pytest.mark.parametrize("mode", [0, 1, 2, 4, 8, 201, 202, 204, 208, -1, -2, -3, -42, -44, -48, -56, -72, -84, -88, -96, -112])   # 100*G + CS; -(40 + W): single-barrier bucket schedule; -(80 + W): + register-resident tables (shared-memory tables when a cloud has more buckets per lane than the registers hold)
 def test_fps_matches_oracle(name, build, ms, mode):
     cl = build()
     xyz, offset, new_offset = _pack(cl, ms)
@@ -62,8 +62,6 @@ def test_fps_matches_oracle(name, build, ms, mode):
     except L.TgnError as e:
         if mode > 0 and "no resident kernel of shape" in str(e):
             pytest.skip("cluster size not applicable to this cloud size")
-        if mode <= -81 and "has no shape" in str(e):
-            pytest.skip("cloud has more buckets per lane than the register-resident kernel holds")
         raise
     torch.cuda.synchronize()
     assert np.array_equal(got.cpu().numpy(), want)

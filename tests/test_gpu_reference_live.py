@@ -1,4 +1,4 @@
-"""GPU parity against the REFERENCE ITSELF running on the same B200: the reference's unmodified
+"""GPU parity against the REFERENCE ITSELF running on the same GPU: the reference's unmodified
 ``pointnet2_utils.py`` / ``pointops.py`` / ``models/modules/*.py`` (staged as ``oracle/_ref/reference_py.tgz`` by
 ``__graft_entry__.build()``, or read from /root/reference) on the verbatim ``pointops`` kernels of ``oracle/_ref``.
 Skipped when that snapshot is absent.  What the CPU fixtures cannot pin -- the reference's CUDA arithmetic
@@ -372,7 +372,7 @@ def test_fused_point_transformer_layer_vs_reference_layer(c, K, n, train_bn):
 
 @pytest.mark.parametrize("train_bn", [True, False])
 def test_fused_transition_down_vs_reference(train_bn):
-    """blocks.TransitionDown (stride 4, :59-79) under no_grad on the tcgen05 layer chain: same sampled points, features within 1e-4 /
+    """blocks.TransitionDown (stride 4, :59-79) under no_grad on the tensor-core layer chain: same sampled points, features within 1e-4 /
     the float64 criterion."""
     name = "models.modules.cbl_point_transformer.blocks"
     p = torch.cat([clouds.dental_arch(6000, 5)[0], clouds.dental_arch(3000, 6)[0]]).cuda()

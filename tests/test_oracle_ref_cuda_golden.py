@@ -1,5 +1,5 @@
 """The CPU oracle against fixtures produced by the reference's OWN CUDA kernels (compiled verbatim
-for sm_100a, run on a B200 by tests/golden/make_ref_cuda_golden.py).  Everything bitwise."""
+for the GPU, run by tests/golden/make_ref_cuda_golden.py).  Everything bitwise."""
 import importlib.util
 import os
 

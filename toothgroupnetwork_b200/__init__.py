@@ -1,4 +1,4 @@
-"""toothgroupnetwork_b200 -- B200-native (sm_100a) point-cloud sampling / neighbour-search /
+"""toothgroupnetwork_b200 -- H100-native (sm_90a) point-cloud sampling / neighbour-search /
 grouping / interpolation / grouped shared-MLP operators behind the operator API of
 limhoyeon/ToothGroupNetwork's ``external_libs/pointops`` and ``external_libs/pointnet2_utils``.
 

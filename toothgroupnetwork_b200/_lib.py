@@ -123,7 +123,7 @@ def load() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise TgnError(
             f"{LIB_PATH} is missing: build it with `python -m toothgroupnetwork_b200.build` "
-            "(nvcc, sm_100a).  toothgroupnetwork_b200 has no CPU / PyTorch fallback.")
+            "(nvcc, sm_90a).  toothgroupnetwork_b200 has no CPU / PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, args in _SIGS.items():
         fn = getattr(lib, name)

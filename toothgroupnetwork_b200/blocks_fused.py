@@ -2,14 +2,13 @@
 
 ``accelerate(blocks_module)`` wraps ``PointTransformerLayer.forward`` (:31-44) and ``TransitionDown.forward`` (:59-79) of an
 imported reference ``blocks`` module: when no gradient is needed (the reference's inference and validation run under
-``torch.no_grad()``) and the shape is one the kernels take, the layer runs on ``csrc/pt_layer.cu`` / the tcgen05 layer chain of
+``torch.no_grad()``) and the shape is one the kernels take, the layer runs on ``csrc/pt_layer.cu`` / the tensor-core layer chain of
 ``csrc/pw_mlp.cu``; otherwise the reference's own code runs, untouched.  Parameters, buffers and ``state_dict`` keys are the
 reference's; BatchNorm keeps torch's semantics (batch statistics in ``train()``, which the reference's inference leaves on,
 running statistics updated with the module's momentum, ``num_batches_tracked`` incremented).
 
 What is saved per transformer layer: two identical kNN searches (one, cached), two grouped (n, K, c) tensors, ~30 torch kernels
-of which three are cuDNN BatchNorms over (n, c, K) views -- 56 % of the kernel time of a tgnet_fps step
-(profiles/r2_launches_tgnet_fwd_bwd.csv).
+of which three are cuDNN BatchNorms over (n, c, K) views -- the largest share of the kernel time of a tgnet_fps step.
 """
 from __future__ import annotations
 
@@ -111,7 +110,7 @@ _td_chains = weakref.WeakKeyDictionary()          # module -> its packed-weight 
 
 def transition_down_forward(td, pxo):
     """blocks.TransitionDown.forward (stride != 1, :59-79): FPS, kNN grouping [xyz_rel | feats], Linear + BatchNorm + ReLU, max over K
-    -- a one-layer set abstraction over kNN neighbourhoods -- on the tcgen05 layer chain (batch statistics included)."""
+    -- a one-layer set abstraction over kNN neighbourhoods -- on the tensor-core layer chain (batch statistics included)."""
     p, x, o = pxo
     host_o = o.cpu().tolist()                                    # the reference reads o[i].item() here too (:64-67)
     n_o, count, prev = [], 0, 0

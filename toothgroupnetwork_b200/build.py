@@ -1,9 +1,9 @@
-"""Build libtgn_b200.so (the C-ABI CUDA library) in-tree for sm_100a.
+"""Build libtgn_b200.so (the C-ABI CUDA library) in-tree for sm_90a (H100).
 
     python -m toothgroupnetwork_b200.build [--force] [--jobs N]
 
 nvcc cross-compiles without a GPU; the resulting ``toothgroupnetwork_b200/_lib/libtgn_b200.so``
-is git-ignored but travels to the GPU box with the gpurun snapshot.  sm_100a is the only target.
+is a git-ignored build product.  sm_90a is the only target.
 """
 from __future__ import annotations
 
@@ -19,10 +19,10 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(OUT_DIR, "libtgn_b200.so")
-SOURCES = ["lib.cu", "fps.cu", "fps_bucket.cu", "knn.cu", "knn_grid.cu", "crop_knn.cu", "gather.cu", "csr.cu", "ballquery.cu", "ballquery_grid.cu", "sa_mlp.cu", "sa_mlp_tc.cu", "sa_mlp_tc8.cu", "sa_mlp_tcw.cu", "pw_mlp.cu", "pt_layer.cu", "dbscan.cu"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-    "-Xcompiler", "-fPIC",
+SOURCES = ["lib.cu", "fps.cu", "fps_bucket.cu", "knn.cu", "knn_grid.cu", "crop_knn.cu", "gather.cu", "csr.cu", "ballquery.cu", "ballquery_grid.cu", "sa_mlp.cu", "sa_mlp_tc.cu", "sa_mlp_tcw.cu", "pw_mlp.cu", "pt_layer.cu", "dbscan.cu"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + [
+    "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
     "-I" + os.path.join(ROOT, "include"), "-I" + CSRC,
 ]
 
@@ -39,8 +39,15 @@ def _newest_source_mtime() -> float:
     return max(os.path.getmtime(p) for p in paths)
 
 
+STAMP = os.path.join(OUT_DIR, "gencode.txt")       # the target the library in _lib/ was built for
+
+
 def is_fresh() -> bool:
-    return os.path.exists(LIB) and os.path.getmtime(LIB) >= _newest_source_mtime()
+    """Built from the current sources AND for the current target (a library left from another architecture is rebuilt)."""
+    if not (os.path.exists(LIB) and os.path.getmtime(LIB) >= _newest_source_mtime() and os.path.exists(STAMP)):
+        return False
+    with open(STAMP) as f:
+        return f.read().strip() == " ".join(GENCODE)
 
 
 def build(force: bool = False, jobs: int = 0, verbose: bool = False) -> str:
@@ -65,11 +72,13 @@ def build(force: bool = False, jobs: int = 0, verbose: bool = False) -> str:
 
     with cf.ThreadPoolExecutor(max_workers=jobs or min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB + ".tmp"] + objs
+    link = [nvcc, "-shared"] + GENCODE + ["-o", LIB + ".tmp"] + objs
     res = subprocess.run(link, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError(f"link failed:\n{res.stdout}\n{res.stderr}")
     os.replace(LIB + ".tmp", LIB)
+    with open(STAMP, "w") as f:
+        f.write(" ".join(GENCODE) + "\n")
     return LIB
 
 

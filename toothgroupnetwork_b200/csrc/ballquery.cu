@@ -1,4 +1,4 @@
-// ballquery.cu -- ball query and 3-NN on the PointNet++ side, sm_100a.
+// ballquery.cu -- ball query and 3-NN on the PointNet++ side, sm_90a.
 //
 // The reference has no kernel here: query_ball_point materialises an (S,N) fp32 distance
 // matrix through a K=3 matmul plus an (S,N) int64 index tensor and SORTS every row
@@ -24,8 +24,8 @@ namespace {
 
 constexpr int kTile = 1024;   // points staged per shared-memory tile (16 KB as SoA x,y,z,|p|^2)
 
-// |p|^2 as torch.sum(p ** 2, -1) rounds it ON THE GPU (square_distance :39-40), measured on B200 / torch 2.11
-// (scripts/diag_sumsq.py, profiles/r2_parity.md): a strided reduction (the permuted views the reference's modules
+// |p|^2 as torch.sum(p ** 2, -1) rounds it ON THE GPU (square_distance :39-40), measured with torch 2.11
+// (scripts/diag_sumsq.py): a strided reduction (the permuted views the reference's modules
 // pass) accumulates in index order, (x*x + y*y) + z*z -- the same as torch on the CPU; a CONTIGUOUS (..., 3) tensor
 // (e.g. new_xyz fresh out of index_points) goes through the vectorised reduce path and comes out as
 // (x*x + z*z) + y*y.  `alt` selects the second form; the Python layer derives it from the layout the reference's
@@ -39,6 +39,18 @@ __device__ __forceinline__ float sq_dist_expanded(float ax, float ay, float az, 
     float dot = __fmul_rn(ax, bx);
     dot = __fmaf_rn(ay, by, dot);
     dot = __fmaf_rn(az, bz, dot);
+    float d = __fmul_rn(-2.0f, dot);
+    d = __fadd_rn(d, an);
+    return __fadd_rn(d, bn);
+}
+
+// The same when the reference's matmul has a single column (one dst point per batch, tsegnet.get_ddf): cuBLAS on H100 then
+// takes a matrix-vector path that rounds the dot product as fma(ay, by, ax*bx) + az*bz (measured with torch 2.11 / cuBLAS
+// for CUDA 12.8; two or more columns round as the fused chain above).
+__device__ __forceinline__ float sq_dist_expanded_one_column(float ax, float ay, float az, float an, float bx, float by, float bz,
+                                                             float bn) {
+    float dot = __fmaf_rn(ay, by, __fmul_rn(ax, bx));
+    dot = __fadd_rn(dot, __fmul_rn(az, bz));
     float d = __fmul_rn(-2.0f, dot);
     d = __fadd_rn(d, an);
     return __fadd_rn(d, bn);
@@ -100,8 +112,7 @@ ball_query_kernel(int N, int S, float r2, int nsample, const float* __restrict__
             // four 32-point steps per trip: 16 shared loads issued together, one early-exit test per 128
             // points (the tile arrays are padded to a multiple of 128 with points that can never hit)
             // Each lane tests the ADJACENT points 2*lane and 2*lane+1 of a 64-point step with packed
-            // fp32x2 arithmetic (FMUL2/FFMA2/FADD2: same IEEE-rn results per element, half the issue
-            // slots of an issue-bound kernel); two steps per trip.
+            // fp32 pair arithmetic (same IEEE-rn results per element as scalar code); two steps per trip.
             const uint64_t AX = pack2(ax, ax), AY = pack2(ay, ay), AZ = pack2(az, az), AN = pack2(an, an);
             const uint64_t M2 = pack2(-2.0f, -2.0f);
             const unsigned lt = (1u << lane) - 1u;
@@ -283,7 +294,8 @@ square_distance_kernel(int N, int M, const float* __restrict__ src, const float*
     for (int j = blockIdx.x * 256 + threadIdx.x; j < M; j += gridDim.x * 256) {
         const float* p = dst + 3 * (static_cast<size_t>(b) * M + j);
         const float bx = __ldg(p), by = __ldg(p + 1), bz = __ldg(p + 2);
-        row[j] = sq_dist_expanded(ax, ay, az, an, bx, by, bz, sq_norm_unfused(bx, by, bz, order & 2));
+        const float bn = sq_norm_unfused(bx, by, bz, order & 2);
+        row[j] = M == 1 ? sq_dist_expanded_one_column(ax, ay, az, an, bx, by, bz, bn) : sq_dist_expanded(ax, ay, az, an, bx, by, bz, bn);
     }
 }
 
@@ -302,7 +314,7 @@ int tgn_ball_query(int B, int N, int S, float r2, int nsample, const float* xyz,
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int order = (idx64 >> 4) & 3;      // bit 4: |new_xyz|^2 in the contiguous-reduce order, bit 5: |xyz|^2 likewise
     // Streaming variant (pack once into stream-ordered scratch, then fully independent warps).  Measured
-    // on B200 it ties with the shared-memory tile kernel at 24k points (both issue-bound) and loses
+    // it ties with the shared-memory tile kernel at 24k points (both issue-bound) and loses
     // to its packed-fp32x2 form, so it is only taken on request (idx64 bit 1 set: experiments).
     if (idx64 & 2) {
         keep_async_pool();

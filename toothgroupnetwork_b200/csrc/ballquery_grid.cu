@@ -1,4 +1,4 @@
-// ballquery_grid.cu -- ball query through a uniform grid, for clouds whose balls are sparse (sm_100a).
+// ballquery_grid.cu -- ball query through a uniform grid, for clouds whose balls are sparse (sm_90a).
 //
 // query_ball_point (external_libs/pointnet2_utils/pointnet2_utils.py:120-144) returns, per query, the
 // nsample SMALLEST point indices whose expanded-form distance satisfies !(d > r2), padded with the
@@ -59,8 +59,8 @@ __device__ __forceinline__ int cell_of(float v, float origin, float inv, int dim
 // Per cloud: does the grid pay?  A subsample of <= kEstPoints points is binned into cells of the
 // query radius; the mean population of a point's 27-cell neighbourhood (scaled back to the full cloud)
 // estimates the candidates a grid query tests, and from it the length of the index-order scan the
-// tile kernel needs to collect nsample members.  Cost models in ns per query, fitted on B200
-// (scripts/ball_sweep.py): tile = 3.7e-3 * nsample * N / cand (at most the full scan, 5.6e-4 * N),
+// tile kernel needs to collect nsample members.  Cost models in ns per query, to be refitted on
+// the target GPU with scripts/ball_sweep.py: tile = 3.7e-3 * nsample * N / cand (at most the full scan, 5.6e-4 * N),
 // grid = 1.4 + N * (0.5e-4 + 0.5e-4 * 1024 / S) + 8.6e-4 * cand, with a 15 % bias towards the tile kernel.
 constexpr int kET = 256;
 constexpr int kEstPoints = 4096;

@@ -1,6 +1,6 @@
-// common.cuh -- sm_100a device primitives shared by the kernels of libtgn_b200.so.
-// Everything here is inline PTX for Blackwell (compile with
-// -gencode arch=compute_100a,code=sm_100a); there is no other target.
+// common.cuh -- sm_90a device primitives shared by the kernels of libtgn_b200.so.
+// Everything here is inline PTX for Hopper (compile with
+// -gencode arch=compute_90a,code=sm_90a); there is no other target.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -17,9 +17,9 @@ int sm_count();                       // of the current device (cached per devic
 int ensure_dynamic_smem(const void* func, size_t bytes);   // per (device, kernel) opt-in to > 48 KB of dynamic shared memory
 void keep_async_pool();               // configure the default cudaMallocAsync pool to cache freed scratch
 
-// ---------------------------------------------------------------- packed fp32x2 (FADD2/FMUL2/FFMA2)
-// Each lane of a packed op is an IEEE round-to-nearest fp32 operation, so a sequence of packed
-// ops is bit-identical to the same sequence of scalar ops on either half.
+// ---------------------------------------------------------------- fp32 pairs
+// A pair of floats carried in one 64-bit value.  Each op is two IEEE round-to-nearest fp32 operations, so a
+// sequence of pair ops is bit-identical to the same sequence of scalar ops on either half.
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -29,30 +29,31 @@ __device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t sub2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    unpack2(a, a0, a1);
+    unpack2(b, b0, b1);
+    return pack2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    unpack2(a, a0, a1);
+    unpack2(b, b0, b1);
+    return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
+    float a0, a1, b0, b1;
+    unpack2(a, a0, a1);
+    unpack2(b, b0, b1);
+    return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    float a0, a1, b0, b1, c0, c1;
+    unpack2(a, a0, a1);
+    unpack2(b, b0, b1);
+    unpack2(c, c0, c1);
+    return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
-__device__ __forceinline__ float max3(float a, float b, float c) {
-    float r;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // ---------------------------------------------------------------- shared-memory addresses / clusters
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

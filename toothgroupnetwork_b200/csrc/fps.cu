@@ -1,4 +1,4 @@
-// fps.cu -- farthest point sampling for sm_100a.
+// fps.cu -- farthest point sampling for sm_90a.
 //
 // Replaces pointops/src/sampling/sampling_cuda_kernel.cu:14-171 of the reference (one CTA per
 // cloud re-streaming xyz+tmp from L2 every iteration, 11 block barriers per iteration).
@@ -7,7 +7,7 @@
 //  * A thread-block CLUSTER of CS CTAs owns G clouds at a time.  Every point (x,y,z and its
 //    running minimum t) lives in REGISTERS for the whole kernel: thread u holds SLOTS points of
 //    each cloud, packed two per 64-bit register so the distance update runs on
-//    FADD2/FMUL2/FFMA2.  HBM is touched once to load the clouds and once per sample for idx.
+//    paired fp32 ops.  HBM is touched once to load the clouds and once per sample for idx.
 //  * The argmax is tracked inside the update loop on the ALU pipe (FSETP/FMNMX/SEL run beside the
 //    FP32 pipe, which is the bottleneck: 6 lane-ops per point-update), so no thread ever
 //    re-scans its registers.
@@ -445,7 +445,8 @@ int fps_dispatch(int b, int n_max, const float* xyz, const int* offset, const in
         if (n_max > fps_bucket_max_points()) { set_error("furthestsampling: n_max=%d exceeds the bucket kernel", n_max); return TGN_ERR_INVALID; }
         return fps_bucket_launch(b, n_max, xyz, offset, new_offset, tmp, idx, bs_log2, 100 + (mode == -3 ? 0 : -mode - 40), stream);
     }
-    // mode -(80 + W): single barrier AND register-resident bucket tables (fps_bucket_kernel3; clouds of up to 4 buckets per lane).
+    // mode -(80 + W): single barrier AND register-resident bucket tables (fps_bucket_kernel3; clouds with more buckets per lane
+    // than the registers hold keep the tables in shared memory).
     if (mode <= -81 && mode >= -112) {
         if (n_max > fps_bucket_max_points()) { set_error("furthestsampling: n_max=%d exceeds the bucket kernel", n_max); return TGN_ERR_INVALID; }
         return fps_bucket_launch(b, n_max, xyz, offset, new_offset, tmp, idx, bs_log2, 200 + (-mode - 80), stream);
@@ -461,7 +462,7 @@ int fps_dispatch(int b, int n_max, const float* xyz, const int* offset, const in
         const int sms = sm_count();
         // Throughput shape: two clouds pipelined through the smallest cluster that holds them,
         // when there are at least two clouds and the batch can occupy the machine that way.
-        // (measured on B200, profiles/: the pipelined shapes lose to one cloud per 2-CTA cluster at
+        // (the pipelined shapes lose to one cloud per 2-CTA cluster at
         //  24k points because per-warp reduction overhead doubles with the cluster size, so auto
         //  mode does not pick them; they stay reachable through `mode` for experiments)
         if (false && b >= 2) {

@@ -1,4 +1,4 @@
-// fps_bucket.cu -- bucket-pruned farthest point sampling for sm_100a (bit-exact).
+// fps_bucket.cu -- bucket-pruned farthest point sampling for sm_90a (bit-exact).
 //
 // The brute-force FPS update touches every point every iteration although, after a few
 // samples, a new sample only lowers the running minimum of the points NEAR it.  This kernel
@@ -691,8 +691,8 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
 }
 
 // ---- register-resident bucket tables ("v3") --------------------------------------------------------------------------------
-// At small batches (one cloud per SM or fewer) an iteration is a DEPENDENT CHAIN: ncu (profiles/r2_fps_b1_*.csv) shows ~190
-// warp instructions per warp per iteration at ~15 cycles each, 26 % issue utilisation, most samples waiting at the barrier for
+// At small batches (one cloud per SM or fewer) an iteration is a DEPENDENT CHAIN: a profile shows
+// ~190 warp instructions per warp per iteration, low issue utilisation, most samples waiting at the barrier for
 // the warp that had a bucket to update.  v3 keeps the single barrier of v2 and shortens the chain: the table entries of a
 // warp's OWN buckets (box, skip threshold, candidate value / key / coordinates: 12 registers per bucket, BPL buckets per lane)
 // never leave registers -- box tests need no shared-memory loads, an update hands the new candidate to the owner lane with
@@ -905,12 +905,11 @@ int fps_bucket_launch(int b, int n_max, const float* xyz, const int* offset, con
         // redundant per-warp steps and cheaper barriers per cloud, more clouds in flight to hide latency).
         const int sms = sm_count();
         auto fits = [&](int per_sm) { return static_cast<size_t>(per_sm) * (smem + 1024) <= 220 * 1024; };
-        // Auto (shape 0).  Measured on B200, 24k-point clouds -> 1024 samples (profiles/r2_fps_modes.json): up to 4 clouds per SM
-        // the single-barrier kernel with register-resident tables at 16 warps per cloud wins (1.02 ms against 1.62 ms per call
-        // up to one cloud per SM, 3.16 against 3.32 at four); beyond that the batch is DRAM-bound and the three-barrier kernel
-        // at 4 warps per cloud, 8 clouds per SM, stays ahead (5.27 against 6.17 ms per 1184 clouds).
+        // Auto (shape 0), 24k-point clouds -> 1024 samples: up to 4 clouds per SM the single-barrier kernel with register-resident
+        // tables at 16 warps per cloud; beyond that the batch is DRAM-bound and the three-barrier kernel at 4 warps per cloud,
+        // 8 clouds per SM, is used.
         // Raw meshes (one cloud of 1e5..2e5 vertices -> 24 000, gen_utils.py:135-140): the same kernel with 4-8 buckets per lane
-        // while every cloud can have an SM to itself (profiles/r2_raw_mesh_fps.json).
+        // while every cloud can have an SM to itself.
         if (shape == 0 && ((b <= 4 * sms && ws.nbmax <= 2 * 512) || (b <= sms && ws.nbmax <= 8 * 512))) shape = 200 + 16;
         const bool v2 = shape >= 100 && shape < 200;          // 100 + W: the single-barrier schedule (fps_bucket_kernel2)
         const bool v3 = shape >= 200;                         // 200 + W: the same with register-resident bucket tables (fps_bucket_kernel3)
@@ -931,7 +930,17 @@ int fps_bucket_launch(int b, int n_max, const float* xyz, const int* offset, con
             else if (warps == 4 && bpl <= 2) rc = launch_main3<128, 2>(b, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream);
             else if (warps == 4 && bpl <= 3) rc = launch_main3<128, 3>(b, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream);
             else if (warps == 4 && bpl <= 4) rc = launch_main3<128, 4>(b, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream);
-            if (rc == -1) { set_error("furthestsampling: bucket kernel v3 has no shape of %d warps x %d buckets per lane", warps, bpl); rc = TGN_ERR_INVALID; }
+            // more buckets per lane than the registers of this CTA width hold: the same single-barrier schedule with the
+            // tables in shared memory (fps_bucket_kernel2, bitwise the same samples)
+            if (rc == -1) {
+                switch (warps) {
+                    case 32: rc = launch_main2<1024>(b, smem, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream); break;
+                    case 16: rc = launch_main2<512>(b, smem, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream); break;
+                    case 8: rc = launch_main2<256>(b, smem, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream); break;
+                    case 4: rc = launch_main2<128>(b, smem, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream); break;
+                    default: set_error("furthestsampling: bucket kernel v3 has no shape of %d warps x %d buckets per lane", warps, bpl); rc = TGN_ERR_INVALID;
+                }
+            }
         } else if (v2) {
             switch (warps) {
                 case 16: rc = launch_main2<512>(b, smem, xyz, offset, new_offset, tmp, idx, ws, bs_log2, stream); break;

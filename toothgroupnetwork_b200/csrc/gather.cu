@@ -1,4 +1,4 @@
-// gather.cu -- the gather / scatter family of the pointops API for sm_100a.
+// gather.cu -- the gather / scatter family of the pointops API for sm_90a.
 //
 // Replaces pointops/src/{grouping,interpolation,subtraction,aggregation}/*_cuda_kernel.cu of
 // the reference (one thread per output ELEMENT, three integer divisions and one index load per

@@ -1,4 +1,4 @@
-// knn.cu -- segment-aware k nearest neighbours for sm_100a.
+// knn.cu -- segment-aware k nearest neighbours for sm_90a.
 //
 // Replaces pointops/src/knnquery/knnquery_cuda_kernel.cu:65-116 of the reference (one THREAD
 // per query, a 100-entry max-heap in local memory -- 800 B of stack per thread -- and a

@@ -78,11 +78,11 @@ int sm_count()
 {
     static std::atomic<int> cached[64];                   // per device, 0 = unknown
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 148; }
+    if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); return 132; }   // H100 SXM
     std::atomic<int>& slot = cached[dev & 63];
     int n = slot.load(std::memory_order_relaxed);
     if (n == 0) {
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { (void)cudaGetLastError(); n = 148; }   // B200
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { (void)cudaGetLastError(); n = 132; }   // H100 SXM
         slot.store(n, std::memory_order_relaxed);
     }
     return n;

@@ -2,8 +2,8 @@
 // SURVEY.md 8(f)-3.
 //
 // The reference builds, per layer, two grouped (n, K, c) tensors with two identical kNN searches, and runs ~30 torch kernels
-// over them: three BatchNorms on (n, c, K)-shaped views (cudnn::bn_fw_tr_1C11: 56 % of the kernel time of a tgnet_fps step,
-// profiles/r2_launches_tgnet_fwd_bwd.csv), four small Linears, a softmax over K and the share-planes aggregation.
+// over them: three BatchNorms on (n, c, K)-shaped views (cudnn::bn_fw_tr_1C11, the largest
+// share of the kernel time of a tgnet_fps step), four small Linears, a softmax over K and the share-planes aggregation.
 // Its inference runs those BatchNorms on BATCH statistics (no .eval(), SURVEY 3c), so one fused kernel is not valid; this file
 // is the multi-pass form.  For query i and neighbour j (nbr = idx[i, j]) everything is a function of a handful of gathers:
 //

@@ -1,4 +1,4 @@
-// pw_mlp.cu -- 1x1-convolution chains with BATCH-STATISTICS BatchNorm on tcgen05 (any width).
+// pw_mlp.cu -- 1x1-convolution chains with BATCH-STATISTICS BatchNorm on warpgroup MMAs (any width).
 //
 // Every reference call site of a set-abstraction / feature-propagation MLP runs BatchNorm in training mode,
 // inference included (SURVEY.md 3c: the inference pipelines never call .eval()), i.e. layer l+1 cannot start
@@ -15,24 +15,26 @@
 //   * layer 0 of a set abstraction builds its operand straight from the neighbourhood gather
 //     ([feats | xyz - centre] or [xyz - centre | feats]); layer 0 of a feature propagation reads up to two strided
 //     segments (skip features channel-first, interpolated features point-major): no grouped tensor, no concat;
-//   * the GEMM runs TRANSPOSED (weights = M side, rows = N side) so that a TMEM lane is an output channel: the
-//     per-channel sum / sum^2 (fp64 atomics, two per channel per CTA), and for the last set-abstraction layer the
+//   * the GEMM runs TRANSPOSED (weights = M side, rows = N side); after the K loop the accumulators are staged
+//     channel-major in shared memory, so that in the epilogue a thread owns one output channel: the per-channel
+//     sum / sum^2 (fp64 atomics, two per channel per CTA), and for the last set-abstraction layer the
 //     per-neighbourhood max AND min over the K rows (BN's scale may be negative, so both are kept), are
 //     loops inside one thread; the last SA layer never writes its (rows x C) pre-activation at all;
 //   * arithmetic: batch-statistics BatchNorm amplifies rounding differences (a channel whose variance is small is
 //     scaled up by 1/sqrt(var)), so this engine is fp32-GRADE: both operands are split into THREE bf16 parts
-//     (x = x1 + x2 + x3 exactly: 3 x 8 = 24 significand bits) and six kind::f16 MMAs per K-step accumulate every
-//     product term down to 2^-16 of the leading one (x1w1, x1w2, x2w1, x2w2, x1w3, x3w1) into fp32 TMEM
+//     (x = x1 + x2 + x3 exactly: 3 x 8 = 24 significand bits) and six bf16 MMAs per K-step accumulate every
+//     product term down to 2^-16 of the leading one (x1w1, x1w2, x2w1, x2w2, x1w3, x3w1) into fp32
 //     accumulators; what is dropped (x2w3, x3w2, x3w3) is ~2^-23 per product, the size of an fp32 rounding.
 //     `precision` 2 keeps two parts and three MMAs (~2^-16 per product, ~1e-5 end to end) for callers that do
 //     not need more (eval-mode BatchNorm);
-//   * weights are pre-split once per parameter version into the canonical K-major UMMA layout, one contiguous
-//     24 KB block per (128-channel tile, 32-wide K chunk), and fetched by the TMA engine with ONE
-//     cp.async.bulk per pipeline stage completing on the stage's mbarrier (SASS: UBLKCP); the activation
-//     side of the stage is produced by 256 threads (one row each) which arrive on the same barrier.
+//   * weights are pre-split once per parameter version into the canonical K-major no-swizzle layout, one
+//     contiguous 24 KB block per (128-channel tile, 32-wide K chunk), and fetched by the TMA engine with ONE
+//     cp.async.bulk per pipeline stage completing on the stage's mbarrier; the activation side of the stage is
+//     produced by the 256 threads of the CTA (one row each).
 //
-// Pipeline per CTA (tile = 128 output channels x 256 rows): 8 producer/epilogue warps + 1 MMA warp,
-// kStages stages of {weights 24 KB | activations 48 KB}, full/empty mbarriers, tcgen05.commit releases a stage.
+// Pipeline per CTA (tile = 128 output channels x 256 rows): two warpgroups, warpgroup j owns output channels
+// 64j..64j+63 of the tile (one m64n256 accumulator, 128 registers per thread).  Two stages of {weights 24 KB |
+// activations 48 KB}: while the MMAs of K chunk k run asynchronously, the same threads build the operand of chunk k+1.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -47,22 +49,23 @@ namespace {
 
 using namespace tc;
 
-constexpr int kMT = 128;                 // output channels per tile (M of the MMA, TMEM lanes)
-constexpr int kNT = 256;                 // rows per tile (N of the MMA, TMEM columns)
+constexpr int kMT = 128;                 // output channels per tile (M of the MMAs: two 64-channel warpgroup slices)
+constexpr int kNT = 256;                 // rows per tile (N of the MMA)
 constexpr int kKC = 32;                  // K per pipeline stage (two K=16 MMA steps)
-constexpr int kProducers = kNT;          // one producer thread per row
-constexpr int kThreads = kProducers + 32;
+constexpr int kThreads = kNT;            // one producer thread per row; two consumer warpgroups
 constexpr int kParts = 3;                                // bf16 parts per operand
 constexpr uint32_t kWPart = kMT * kKC * 2;               // bytes of one part of a packed weight block (8 KB)
 constexpr uint32_t kWBlock = kWPart * kParts;            // 24 KB
 constexpr uint32_t kXPart = kNT * kKC * 2;               // bytes of one part of the activation side of a stage (16 KB)
 constexpr uint32_t kStageBytes = kWBlock + kParts * kXPart;   // 72 KB
-constexpr int kMaxStages = 3;
+constexpr int kStages = 2;
+constexpr int kYStride = kNT + 1;                        // floats per channel of the staged accumulator tile: odd, so the 32
+                                                         // channels a warp reads at one column fall in 32 different banks
+static_assert(kMT * kYStride * 4 <= kStages * kStageBytes, "the staged accumulator tile reuses the stage buffers");
 
 struct PwArgs {
     tgn_pw_layer_t L;
     int nkc;                 // K chunks
-    int stages;
     uint32_t off_affine;     // float4[cin] (mean_hi, mean_lo, scale, beta) when in_affine != 0
     uint32_t off_bars;
     uint32_t smem_total;
@@ -134,22 +137,11 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int r0 = blockIdx.x * kNT;               // first row of the tile
     const int m0 = blockIdx.y * kMT;               // first output channel of the tile
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + a.off_bars);
-    const uint32_t bar_full = sbase + a.off_bars + 16;                 // kMaxStages x 8
-    const uint32_t bar_empty = bar_full + 8 * kMaxStages;
-    const uint32_t bar_acc = bar_empty + 8 * kMaxStages;
+    const uint32_t bar_full = sbase + a.off_bars;                      // kStages x 8: weights of the stage have landed
     float4* affine = reinterpret_cast<float4*>(smem + a.off_affine);
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + a.off_bars), "r"(kNT) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     if (tid == 0) {
-        for (int s = 0; s < a.stages; ++s) {
-            mbar_init(bar_full + 8 * s, kProducers + 1);
-            mbar_init(bar_empty + 8 * s, 1);
-        }
-        mbar_init(bar_acc, 1);
+        for (int s = 0; s < kStages; ++s) mbar_init(bar_full + 8 * s, 1);
         mbar_fence_init();
     }
     // ---- input BatchNorm (of the previous layer) -> per-channel scale / shift ------------------------------
@@ -160,17 +152,16 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
                                        L.in_running_var);
         }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     if (L.in_affine == 1 && L.in_update_running && blockIdx.x == 0 && blockIdx.y == 0) {
         for (int c = tid; c < L.cin; c += kThreads)
             bn_update_running(c, L.cin, L.in_stats, static_cast<double>(L.rows), L.in_momentum, L.in_running_mean, L.in_running_var);
     }
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp < kProducers / 32) {
-        // =========================== producers: one row each ==================================================
+    float acc[kNT / 2];              // D^T[m0 + 64 wg + .., r0 + ..] of this thread's warpgroup wg
+#pragma unroll
+    for (int i = 0; i < kNT / 2; ++i) acc[i] = 0.f;
+    {
+        // =========================== producers: one row each; MMAs: one 64-channel slice per warpgroup ==========
         const int r = r0 + tid;
         const bool valid = r < L.rows;
         // source addressing of this row
@@ -203,10 +194,11 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
         const long long cs0 = L.seg_chan_stride[0], cs1 = L.seg_chan_stride[1];
         const int feat_lo = L.xyz_first ? 3 : 0;                      // channel of feats[0]
         const int rel_lo = L.xyz_first ? 0 : L.D;                     // channel of rel0
+        const int wg = warp >> 2;
         for (int kc = 0; kc < a.nkc; ++kc) {
-            const int s = kc % a.stages;
-            const uint32_t use = kc / a.stages;
-            if (use > 0) mbar_wait(bar_empty + 8 * s, (use - 1) & 1);
+            // stage s was last read by the MMAs of chunk kc - 2, which both warpgroups have waited for (end of the
+            // previous iteration)
+            const int s = kc % kStages;
             const uint32_t stage = sbase + s * kStageBytes;
             if (tid == 0) {
                 mbar_arrive_expect_tx(bar_full + 8 * s, kWBlock);
@@ -260,17 +252,55 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
                 st_shared_v4(x1 + 2 * kXPart + j * (kNT * 16), p3[0], p3[1], p3[2], p3[3]);
             }
             proxy_fence_async();
-            mbar_arrive(bar_full + 8 * s);
+            __syncthreads();                                  // the activation side of the stage is complete
+            mbar_wait(bar_full + 8 * s, (kc / kStages) & 1);  // ... and its weights have landed
+            fence_regs(acc);
+            wgmma_fence();
+            const uint32_t w0 = stage + wg * 64 * 16, x0 = stage + kWBlock;
+#pragma unroll
+            for (int ks = 0; ks < kKC / 16; ++ks) {
+                uint64_t dw[kParts], dx[kParts];
+#pragma unroll
+                for (int i = 0; i < kParts; ++i) {
+                    dw[i] = make_smem_desc(w0 + i * kWPart + ks * 2 * (kMT * 16), kMT * 16);
+                    dx[i] = make_smem_desc(x0 + i * kXPart + ks * 2 * (kNT * 16), kNT * 16);
+                }
+                wgmma_bf16<kNT>(acc, dw[0], dx[0], kc > 0 || ks > 0);
+                wgmma_bf16<kNT>(acc, dw[0], dx[1], true);
+                wgmma_bf16<kNT>(acc, dw[1], dx[0], true);
+                if (L.precision != 2) {
+                    wgmma_bf16<kNT>(acc, dw[1], dx[1], true);
+                    wgmma_bf16<kNT>(acc, dw[0], dx[2], true);
+                    wgmma_bf16<kNT>(acc, dw[2], dx[0], true);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                                  // the MMAs of chunk kc - 1 are complete in this warpgroup,
+            fence_regs(acc);
+            __syncthreads();                                  // ... and in the other one: stage (kc + 1) % 2 is free
         }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        __syncthreads();                                      // every MMA is complete: the stage buffers are free
+        // accumulators -> channel-major tile in the (now idle) stage buffers
+        float* ytile = reinterpret_cast<float*>(smem);
+        const int ch = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < kNT / 8; ++i) {
+            const int col = 8 * i + 2 * (lane & 3);
+            ytile[ch * kYStride + col] = acc[4 * i];
+            ytile[ch * kYStride + col + 1] = acc[4 * i + 1];
+            ytile[(ch + 8) * kYStride + col] = acc[4 * i + 2];
+            ytile[(ch + 8) * kYStride + col + 1] = acc[4 * i + 3];
+        }
+        __syncthreads();
 
         // =========================== epilogue: thread = output channel ======================================
-        mbar_wait_suspend(bar_acc, 0);
-        tc_fence_after();
         const int q = warp & 3, half = warp >> 2;
         const int c = m0 + 32 * q + lane;
         const bool c_ok = c < L.cout;
         const float bias = (c_ok && L.bias) ? __ldg(L.bias + c) : 0.f;
-        const uint32_t trow = tmem_base + (static_cast<uint32_t>(32 * q) << 16) + half * (kNT / 2);
+        const float* trow = ytile + (32 * q + lane) * kYStride + half * (kNT / 2);
         double s1 = 0.0, s2 = 0.0;
         const int G = L.group;
         float gmax = -INFINITY, gmin = INFINITY;
@@ -280,7 +310,8 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
             const int rb = col_lo + cb;                       // global row of the block's first column
             if (rb >= L.rows) break;                          // warp-uniform
             uint32_t v[32];
-            tmem_ld32(trow + cb, v);
+#pragma unroll
+            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(trow[cb + i]);
             const int nvalid = min(32, L.rows - rb);
             float f1 = 0.f, f2 = 0.f;
 #pragma unroll
@@ -331,45 +362,6 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
             atomicAdd(L.stats + c, s1);
             atomicAdd(L.stats + L.cout + c, s2);
         }
-        tc_fence_before();
-    } else {
-        // =========================== MMA issuer (one warp, one elected lane) ===============================
-        const uint32_t idesc = make_idesc_bf16(kNT);
-        for (int kc = 0; kc < a.nkc; ++kc) {
-            const int s = kc % a.stages;
-            mbar_wait(bar_full + 8 * s, (kc / a.stages) & 1);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t stage = sbase + s * kStageBytes;
-                const uint32_t w0 = stage, x0 = stage + kWBlock;
-#pragma unroll
-                for (int ks = 0; ks < kKC / 16; ++ks) {
-                    uint64_t dw[kParts], dx[kParts];
-#pragma unroll
-                    for (int i = 0; i < kParts; ++i) {
-                        dw[i] = make_smem_desc(w0 + i * kWPart + ks * 2 * (kMT * 16), kMT * 16);
-                        dx[i] = make_smem_desc(x0 + i * kXPart + ks * 2 * (kNT * 16), kNT * 16);
-                    }
-                    mma_bf16_ss(tmem_base, dw[0], dx[0], idesc, kc > 0 || ks > 0);
-                    mma_bf16_ss(tmem_base, dw[0], dx[1], idesc, true);
-                    mma_bf16_ss(tmem_base, dw[1], dx[0], idesc, true);
-                    if (a.L.precision != 2) {
-                        mma_bf16_ss(tmem_base, dw[1], dx[1], idesc, true);
-                        mma_bf16_ss(tmem_base, dw[0], dx[2], idesc, true);
-                        mma_bf16_ss(tmem_base, dw[2], dx[0], idesc, true);
-                    }
-                }
-                mma_commit(bar_empty + 8 * s);                 // stage reusable once these MMAs have read it
-                if (kc == a.nkc - 1) mma_commit(bar_acc);      // accumulator complete
-            }
-            __syncwarp();
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kNT) : "memory");
     }
 }
 
@@ -470,15 +462,10 @@ int tgn_pw_layer_forward(const tgn_pw_layer_t* layer, void* stream)
     }
     a.nkc = (L.cin + kKC - 1) / kKC;
     const uint32_t affine_bytes = L.in_affine ? static_cast<uint32_t>(L.cin) * 16 : 0;
-    int stages = kMaxStages;
-    for (;; --stages) {
-        a.off_affine = stages * kStageBytes;
-        a.off_bars = (a.off_affine + affine_bytes + 15) / 16 * 16;
-        a.smem_total = a.off_bars + 16 + 8 * (2 * kMaxStages + 1);
-        if (a.smem_total <= 227 * 1024 || stages == 2) break;
-    }
+    a.off_affine = kStages * kStageBytes;
+    a.off_bars = (a.off_affine + affine_bytes + 15) / 16 * 16;
+    a.smem_total = a.off_bars + 8 * kStages;
     if (a.smem_total > 227 * 1024) { set_error("pw_layer_forward: cin %d too wide", L.cin); return TGN_ERR_INVALID; }
-    a.stages = std::min(stages, std::max(a.nkc, 1));
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(pw_layer_kernel), 227 * 1024);
     if (rc_attr != TGN_OK) return rc_attr;
     dim3 grid((L.rows + kNT - 1) / kNT, (L.cout + kMT - 1) / kMT);

@@ -10,7 +10,7 @@
 // rows of each group before anything is written: HBM sees the inputs once and (B, C_out, S) once.
 //
 // This engine is exact fp32 FMA arithmetic and handles any K and any widths <= 128; it is the
-// numerical reference for, and the fallback of, the tcgen05 engine in sa_mlp_tc.cu.
+// numerical reference for, and the fallback of, the tensor-core engine in sa_mlp_tc.cu.
 #include <algorithm>
 
 #include "common.cuh"
@@ -50,8 +50,7 @@ __device__ __forceinline__ void gather_rows_to_smem(const SaParams& p, int b, in
 }
 
 // Output columns per warp CPW (kWarps warps): 4 rows x CPW columns per thread.  The accumulators are packed
-// fp32x2 pairs of adjacent output columns (FFMA2: two IEEE fp32 FMAs per issue slot, each rounding like the
-// scalar op -- the scalar FFMA pipe issues every other cycle, so this doubles the FMA rate); the weight pairs
+// fp32 pairs of adjacent output columns (two IEEE fp32 FMAs each, rounding like the scalar op); the weight pairs
 // come straight out of the 16-byte shared loads.
 template <int CPW>
 __device__ __forceinline__ void dense_layer(const float* __restrict__ act_in, float* __restrict__ act_out, const float* wt,
@@ -255,18 +254,13 @@ extern "C" int tgn_sa_group_mlp_max(int B, int N, int S, int K, int D, const flo
     // auto: the 3xTF32 tensor-core engine when the shape fits it (widths <= 64), else the wide tensor-core
     // engine (tf32 first layer, bf16x2-split later layers: ~1e-5 relative, inside the 1e-4 bar), else the
     // exact-FMA CUDA-core engine (any K, widths <= 128)
-    // engine 4: eight tile groups per SM, bf16x3 operands (C_in <= 16, widths <= 64, K in {16, 32}); on request only until
-    // its measured time beats engine 2 on the bench shape (profiles/)
-    if (engine == 4) {
-        if (!sa_mlp_tc8_supported(p)) { set_error("sa_group_mlp_max: shape not supported by the eight-group tcgen05 engine"); return TGN_ERR_INVALID; }
-        return sa_mlp_tc8_launch(p, st);
-    }
+    if (engine < 0 || engine > 5 || engine == 4) { set_error("sa_group_mlp_max: unknown engine %d", engine); return TGN_ERR_INVALID; }
     if (engine == 2 || engine == 5 || (engine == 0 && sa_mlp_tc_supported(p))) {
-        if (!sa_mlp_tc_supported(p)) { set_error("sa_group_mlp_max: shape not supported by the tcgen05 engine"); return TGN_ERR_INVALID; }
+        if (!sa_mlp_tc_supported(p)) { set_error("sa_group_mlp_max: shape not supported by the tensor-core engine"); return TGN_ERR_INVALID; }
         return sa_mlp_tc_launch(p, st, engine == 5 ? 2 : 4);     // 5: half-size CTAs (two per SM; share an SM with other streams' kernels)
     }
     if (engine == 3 || (engine == 0 && sa_mlp_tcw_supported(p))) {
-        if (!sa_mlp_tcw_supported(p)) { set_error("sa_group_mlp_max: shape not supported by the wide tcgen05 engine"); return TGN_ERR_INVALID; }
+        if (!sa_mlp_tcw_supported(p)) { set_error("sa_group_mlp_max: shape not supported by the wide tensor-core engine"); return TGN_ERR_INVALID; }
         return sa_mlp_tcw_launch(p, st);
     }
     return sa_mlp_fp32_launch(p, st);

@@ -32,7 +32,5 @@ bool sa_mlp_tc_supported(const SaParams& p);
 int sa_mlp_tc_launch(SaParams p, cudaStream_t st, int groups_per_cta = 4);
 bool sa_mlp_tcw_supported(const SaParams& p);     // wide hidden layers: tf32 first layer, bf16x2-split later layers
 int sa_mlp_tcw_launch(SaParams p, cudaStream_t st);
-bool sa_mlp_tc8_supported(const SaParams& p);     // eight tile groups per SM, bf16x3 operands: C_in <= 16, widths <= 64, K in {16, 32}
-int sa_mlp_tc8_launch(SaParams p, cudaStream_t st);
 
 }  // namespace tgn

@@ -1,33 +1,25 @@
-// sa_mlp_tc.cu -- tcgen05 (5th-gen tensor core) engine of the fused set-abstraction body.
+// sa_mlp_tc.cu -- warpgroup-MMA (wgmma) tensor-core engine of the fused set-abstraction body.
 //
 // Same contract as the fp32 engine in sa_mlp.cu, but the per-layer contraction
 //      D[128 rows, N] = A[128 rows, K] * W[N, K]^T
-// runs on the tensor cores with the accumulator in TENSOR MEMORY:
-//   * a CTA is 4 independent TILE GROUPS of 128 threads; a group owns one 128-row tile (128/K
-//     neighbourhoods) at a time, thread r of the group owns row r end to end: it gathers its
-//     neighbour's [xyz_rel | feats] row, and after each layer reads ITS accumulator lane back with
-//     tcgen05.ld (32x32b: warp w owns TMEM lanes 32(w%4)..+31), applies bias + ReLU and writes
-//     the next layer's A operand -- the grouped tensor and the inter-layer activations never
-//     leave the SM.  The four groups share the weights but nothing else (own TMEM columns, own
-//     operand buffers, own mbarrier, named barriers instead of __syncthreads), so while one group
-//     waits for its gather or its MMAs the others fill the issue slots and the tensor pipe;
-//   * operands live in shared memory in the canonical K-major, no-swizzle UMMA layout
-//     (8x16-byte core matrices; element (r,k) at (k/4)*LBO + r*16 + (k%4)*4 with SBO = 128 B), which a
-//     row-per-thread writer fills with conflict-free 16-byte stores;
-//   * fp32 fidelity: inputs are split a = a_hi + a_lo with a_hi the tf32 truncation, and each
-//     K-step issues three kind::tf32 MMAs (hi*hi + lo*hi + hi*lo) into the same accumulator
-//     ("3xTF32"), so the result carries ~2^-21 relative error instead of tf32's 2^-10 -- the
-//     reference's own default for these 1x1 convolutions is plain TF32 (SURVEY.md 7.1);
-//   * one elected thread per group issues the MMAs and tcgen05.commit's the group's mbarrier (one
-//     completion per barrier between two waits of any thread: a waiter that could see TWO completions
-//     of the same barrier -- tried: the last layer split in two committed halves -- aliases the phase
-//     parity and deadlocks; the split also cost 15 % through the doubled MMA issue);
-//   * the LAST layer runs transposed, D^T[channel, row] = W[channel, K] * X[row, K]^T: the weights
-//     (zero-padded to 128 channels) are the A operand and the activation tile -- already in the
-//     canonical K-major layout -- is the B operand (N = 128 rows).  A TMEM lane is then an output
-//     channel and its 128 columns are the rows of the tile, so the max over the K rows of a
-//     neighbourhood is a chain of 3-input FMNMX inside ONE thread (no cross-lane reduction, no
-//     partial buffers) and the thread stores the channel-first output directly.
+// runs on the tensor cores with the accumulator in registers:
+//   * a CTA is up to 4 independent TILE GROUPS of 128 threads (one warpgroup each); a group owns one 128-row tile
+//     (128/K neighbourhoods) at a time.  Thread r of the group gathers row r's [xyz_rel | feats] row into the
+//     first layer's operand; each layer then runs as two 64-row wgmma slices, and after each slice the threads
+//     add the bias, apply ReLU and write the next layer's operand from their accumulator fragments -- the grouped
+//     tensor and the inter-layer activations never leave the SM.  The groups share the weights but nothing else
+//     (own operand buffers, named barriers instead of __syncthreads), so while one group waits for its gather or
+//     its MMAs the others fill the issue slots and the tensor pipe;
+//   * operands live in shared memory in the canonical K-major, no-swizzle layout (8x16-byte core matrices;
+//     element (r,k) at (k/4)*LBO + r*16 + (k%4)*4 with SBO = 128 B);
+//   * fp32 fidelity: inputs are split a = a_hi + a_lo with a_hi the tf32 truncation, and each K-step issues
+//     three tf32 MMAs (hi*hi + lo*hi + hi*lo) into the same accumulator ("3xTF32"), so the result carries
+//     ~2^-21 relative error instead of tf32's 2^-10 -- the reference's own default for these 1x1 convolutions is
+//     plain TF32 (SURVEY.md 7.1);
+//   * the LAST layer runs transposed, D^T[channel, row] = W[channel, K] * X[row, K]^T: the weights (zero-padded
+//     to 128 channels) are the A operand and the activation tile is the B operand (N = 128 rows), so a thread's
+//     accumulator fragment holds two channels across all rows of the tile; the max over the K rows of a
+//     neighbourhood is a chain of max inside the thread plus two shuffles across its quad.
 // Weights are split and laid out once per CTA; CTAs are persistent over tiles.
 #include <algorithm>
 
@@ -43,73 +35,63 @@ using namespace tc;
 
 constexpr int kRows = 128;                            // rows of a tile = threads of a tile group
 constexpr int kMaxGroups = 4;                         // tile groups per CTA: 4 (one CTA owns the SM) or 2 (two CTAs per SM, or one
-                                                      // beside another kernel's CTAs: 32K registers / 256 TMEM columns each)
+                                                      // beside another kernel's CTAs: 32K registers each)
 constexpr uint32_t kChunkStrideA = kRows * 16;        // LBO of the A operand: one 16-byte K-chunk of all rows
 
 struct TcLayout {
     int kpad[kSaMaxLayers];          // K of layer l, multiple of 8
     int npad[kSaMaxLayers];          // N of layer l, multiple of 16
-    uint32_t w_hi[kSaMaxLayers], w_lo[kSaMaxLayers], bias[kSaMaxLayers];   // byte offsets in dynamic smem
+    uint32_t w_hi[kSaMaxLayers], w_lo[kSaMaxLayers];   // byte offsets in dynamic smem
     uint32_t a_hi[kMaxGroups], a_lo[kMaxGroups];   // per group activation operands (A of the inner layers, B of the last)
     int groups;                      // tile groups per CTA
-    uint32_t ones;                   // constant [128 x 8] tile that adds the bias through the MMA
-    uint32_t misc;                   // tmem base (u32) @0, group mbarriers (u64) @8+8g
     uint32_t total;
-    uint32_t tmem_cols, group_cols;
     int tiles_per_cloud, gpt;
     uint32_t tpc_magic;              // floor(2^32 / tiles_per_cloud): t / tiles_per_cloud by IMAD.HI + one fix-up
-    int a_tmem;                      // 1: the activation operands of the inner layers live in tensor memory
 };
 
-// Inner-layer epilogue of one thread: its accumulator lane (NP columns) -> bias is already in, ReLU,
-// tf32 hi/lo split, 16-byte stores into the next layer's K-major operand (row r).
+// One inner layer on one 64-row slice (rows 64h..64h+63) of a group's tile: 3xTF32 MMAs, then + bias, ReLU, tf32 hi/lo
+// split and 8-byte stores of the fragment pairs into the next layer's K-major operand (the same buffers: the slice
+// only overwrites its own rows, which no other slice reads).
 template <int NP>
-__device__ __forceinline__ void mid_epilogue(uint32_t tmem_row, uint32_t a_hi, uint32_t a_lo, int r)
+__device__ __forceinline__ void inner_layer(int h, int kp, uint32_t a_hi, uint32_t a_lo, uint32_t w_hi, uint32_t w_lo,
+                                            const float* __restrict__ bias, int cout, int g)
 {
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+    const uint32_t lbo_w = NP * 16;
+    uint64_t d_xhi = make_smem_desc(a_hi + h * 64 * 16, kChunkStrideA), d_xlo = make_smem_desc(a_lo + h * 64 * 16, kChunkStrideA);
+    uint64_t d_whi = make_smem_desc(w_hi, lbo_w), d_wlo = make_smem_desc(w_lo, lbo_w);
+    float acc[NP / 2];
 #pragma unroll
-    for (int c0 = 0; c0 < NP; c0 += 32) {
-        uint32_t v[32];
-        const bool full = NP - c0 >= 32;             // NP is a multiple of 16: a chunk is 32 or 16 wide
-        if (full) tmem_ld32(tmem_row + c0, v);
-        else tmem_ld16(tmem_row + c0, v);
+    for (int i = 0; i < NP / 2; ++i) acc[i] = 0.f;
+    fence_regs(acc);
+    wgmma_fence();
+    for (int ks = 0; ks < kp / 8; ++ks) {
+        wgmma_tf32<NP>(acc, d_xhi, d_whi, ks > 0);
+        wgmma_tf32<NP>(acc, d_xlo, d_whi, true);
+        wgmma_tf32<NP>(acc, d_xhi, d_wlo, true);
+        d_xhi += desc_step(2 * kChunkStrideA); d_xlo += desc_step(2 * kChunkStrideA);
+        d_whi += desc_step(2 * lbo_w); d_wlo += desc_step(2 * lbo_w);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    group_sync(g);                   // every warp's MMAs have read the operand before any row of it is overwritten
+    const int row = h * 64 + w * 16 + (lane >> 2);
 #pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-            if (i < 16 || full) {
-                uint32_t hi[4], lo[4];
+    for (int i = 0; i < NP / 8; ++i) {
+        const int c = 8 * i + 2 * (lane & 3);
+        const float b0 = c < cout ? __ldg(bias + c) : 0.f, b1 = c + 1 < cout ? __ldg(bias + c + 1) : 0.f;
+        const uint32_t off = static_cast<uint32_t>(c >> 2) * kChunkStrideA + (c & 3) * 4;
 #pragma unroll
-                for (int u = 0; u < 4; ++u) split_tf32(fmaxf(__uint_as_float(v[i + u]), 0.f), hi[u], lo[u]);
-                const uint32_t off = static_cast<uint32_t>((c0 + i) >> 2) * kChunkStrideA + r * 16;
-                st_shared_v4(a_hi + off, hi[0], hi[1], hi[2], hi[3]);
-                st_shared_v4(a_lo + off, lo[0], lo[1], lo[2], lo[3]);
-            }
+        for (int e = 0; e < 2; ++e) {
+            uint32_t hi0, lo0, hi1, lo1;
+            split_tf32(fmaxf(acc[4 * i + 2 * e] + b0, 0.f), hi0, lo0);
+            split_tf32(fmaxf(acc[4 * i + 2 * e + 1] + b1, 0.f), hi1, lo1);
+            const uint32_t o = off + (row + 8 * e) * 16;
+            st_shared_v2(a_hi + o, hi0, hi1);
+            st_shared_v2(a_lo + o, lo0, lo1);
         }
     }
-}
-
-// Same epilogue, but the next layer's A operand goes to TENSOR MEMORY: this thread's lane, hi at column
-// col_hi.., lo at col_lo.. (the tensor core then reads the activations without touching shared memory).
-template <int NP>
-__device__ __forceinline__ void mid_epilogue_tmem(uint32_t tmem_row, uint32_t col_hi, uint32_t col_lo)
-{
-#pragma unroll
-    for (int c0 = 0; c0 < NP; c0 += 16) {
-        uint32_t v[32], hi[16], lo[16];
-        tmem_ld16(tmem_row + c0, v);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) split_tf32(fmaxf(__uint_as_float(v[i]), 0.f), hi[i], lo[i]);
-        tmem_st16(tmem_row + col_hi + c0, hi);
-        tmem_st16(tmem_row + col_lo + c0, lo);
-    }
-    tmem_wait_st();
-}
-
-// max(0, v[B], ..., v[B+15]) with 3-input FMNMX
-template <int B>
-__device__ __forceinline__ float relu_max16(const uint32_t (&v)[32]) {
-    float m = max3(0.f, __uint_as_float(v[B]), __uint_as_float(v[B + 1]));
-#pragma unroll
-    for (int i = 2; i < 16; i += 2) m = max3(m, __uint_as_float(v[B + i]), __uint_as_float(v[B + i + 1]));
-    return m;
 }
 
 template <int kGroups>
@@ -122,17 +104,9 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = tid / kRows;                 // tile group
     const int r = tid - g * kRows;             // row inside the tile (inner layers) / output channel (last layer)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + lay.misc);
-    const uint32_t bar = sbase + lay.misc + 8 + 8 * g;
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + lay.misc), "r"(lay.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (r == 0) { mbar_init(bar, 1); mbar_fence_init(); }
     // ---- weights: split into tf32 hi/lo, canonical K-major layout.  Inner layers: B operand
     //      [npad x kpad] (LBO = npad*16); last layer: A operand [128 x kpad] (LBO = 128*16), zero rows
-    //      beyond cout.  SBO = 128 either way.
+    //      beyond cout.  SBO = 128 either way.  Biases are added in fp32 by the epilogues.
     for (int l = 0; l < p.L; ++l) {
         const int cin = p.ch[l], cout = p.ch[l + 1], kp = lay.kpad[l];
         const int np = l == p.L - 1 ? kRows : lay.npad[l];
@@ -145,36 +119,14 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
             *reinterpret_cast<uint32_t*>(smem + lay.w_hi[l] + off) = hi;
             *reinterpret_cast<uint32_t*>(smem + lay.w_lo[l] + off) = lo;
         }
-        // bias as one extra K=8 step: column k=0 holds bias_hi, k=1 bias_lo (rest 0); multiplied by
-        // the constant "ones" tile it adds bias_hi + bias_lo to every row.
-        for (int e = tid; e < np * 8; e += kThreads) {
-            const int n = e >> 3, k = e & 7;
-            uint32_t hi = 0u, lo = 0u;
-            if (n < cout) split_tf32(__ldg(p.bias[l] + n), hi, lo);
-            const uint32_t off = static_cast<uint32_t>(k >> 2) * (np * 16) + n * 16 + (k & 3) * 4;
-            *reinterpret_cast<uint32_t*>(smem + lay.bias[l] + off) = k == 0 ? hi : (k == 1 ? lo : 0u);
-        }
-    }
-    // constant tile [128 x 8]: columns 0 and 1 are 1.0 (exact in tf32), the rest 0
-    for (int e = tid; e < kRows * 8; e += kThreads) {
-        const int rr = e >> 3, k = e & 7;
-        *reinterpret_cast<float*>(smem + lay.ones + static_cast<uint32_t>(k >> 2) * kChunkStrideA + rr * 16 + (k & 3) * 4) =
-            k < 2 ? 1.0f : 0.0f;
     }
     proxy_fence_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot + g * lay.group_cols;                       // this group's accumulator columns
-    const uint32_t tmem_row = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
     const uint32_t a_hi = sbase + lay.a_hi[g], a_lo = sbase + lay.a_lo[g];
-    uint32_t phase = 0;
 
     const int cout_last = p.ch[p.L];
     const int total_tiles = lay.tiles_per_cloud * p.B;
     const int tile_step = gridDim.x * kGroups;
-    const uint64_t desc_a_hi = make_smem_desc(a_hi, kChunkStrideA, 128);
-    const uint64_t desc_a_lo = make_smem_desc(a_lo, kChunkStrideA, 128);
     const int xoff = p.xyz_first ? 0 : p.D;       // first channel of the xyz_rel block
     const int foff = p.xyz_first ? 3 : 0;         // first channel of the feature block
     const int r_div_k = r / p.K;                  // neighbourhood of this thread's row inside a tile
@@ -242,17 +194,7 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
         const int rows = groups * p.K;
 
         // ---- layer-0 operand: this thread's grouped row --------------------------------------------
-        if (fast_rows && lay.a_tmem) {
-            // the 16-wide padded row (registers) -> tf32 hi/lo -> this thread's TMEM lane, columns 96.. / 112..
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) split_tf32(row[i], hi[i], lo[i]);
-            tmem_st16(tmem_row + (kRows - 32), hi);
-            tmem_st16(tmem_row + (kRows - 16), lo);
-            tmem_wait_st();
-            load_row16(tile + tile_step, j_next, row);          // consumed one tile later: latency hidden
-            j_next = load_index(tile + 2 * tile_step);
-        } else if (fast_rows) {
+        if (fast_rows) {
             // the 16-wide padded row was loaded into registers while the previous tile computed
 #pragma unroll
             for (int kc = 0; kc < 4; ++kc) {
@@ -298,151 +240,49 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
 
         for (int l = 0; l < p.L; ++l) {
             const int kp = lay.kpad[l], np = lay.npad[l];
-            const bool last = (l == p.L - 1);
             proxy_fence_async();           // this thread's operand stores -> visible to the tensor core
-            tc_fence_before();
             group_sync(g);
-            if ((warp & 3) == 0) {
-                // The whole first warp of the group runs the issue code (warp-uniform descriptor maths
-                // stays on the uniform datapath); one lane issues.  The start-address field is the low
-                // 14 bits (units of 16 B): a K-step advances it by a constant.
-                tc_fence_after();
-                const int nks = kp / 8;
-                const uint64_t step_x = (2 * kChunkStrideA) >> 4;
-                uint64_t d_xhi = desc_a_hi, d_xlo = desc_a_lo;
-                if (!last) {
-                    // D[row, n] += X[row, k] * W[n, k]
-                    const uint32_t idesc = make_idesc_tf32(np);
-                    const uint32_t lbo_b = static_cast<uint32_t>(np) * 16;
-                    uint64_t d_whi = make_smem_desc(sbase + lay.w_hi[l], lbo_b, 128);
-                    uint64_t d_wlo = make_smem_desc(sbase + lay.w_lo[l], lbo_b, 128);
-                    const uint64_t step_w = (2 * lbo_b) >> 4;
-                    if (lay.a_tmem) {
-                        // A (activations) from tensor memory: hi at column 128 - 2 kp, lo at 128 - kp, 8 columns per K-step
-                        uint32_t t_hi = tmem_base + (kRows - 2 * kp), t_lo = tmem_base + (kRows - kp);
-                        for (int ks = 0; ks < nks; ++ks) {
-                            if (lane == 0) {
-                                mma_tf32_ts(tmem_base, t_hi, d_whi, idesc, ks > 0);
-                                mma_tf32_ts(tmem_base, t_lo, d_whi, idesc, true);
-                                mma_tf32_ts(tmem_base, t_hi, d_wlo, idesc, true);
-                            }
-                            t_hi += 8; t_lo += 8; d_whi += step_w; d_wlo += step_w;
-                        }
-                    } else {
-                        for (int ks = 0; ks < nks; ++ks) {
-                            if (lane == 0) {
-                                mma_tf32_ss(tmem_base, d_xhi, d_whi, idesc, ks > 0);
-                                mma_tf32_ss(tmem_base, d_xlo, d_whi, idesc, true);
-                                mma_tf32_ss(tmem_base, d_xhi, d_wlo, idesc, true);
-                            }
-                            d_xhi += step_x; d_xlo += step_x; d_whi += step_w; d_wlo += step_w;
-                        }
-                    }
-                    if (lane == 0) {
-                        mma_tf32_ss(tmem_base, make_smem_desc(sbase + lay.ones, kChunkStrideA, 128),
-                                    make_smem_desc(sbase + lay.bias[l], lbo_b, 128), idesc, true);     // + bias
-                        mma_commit(bar);   // arrives on the group's mbarrier when the MMAs above have completed
-                    }
-                } else {
-                    // D^T[channel, row] += W[channel, k] * X[row, k]
-                    const uint32_t idesc = make_idesc_tf32(kRows);
-                    uint64_t d_whi = make_smem_desc(sbase + lay.w_hi[l], kChunkStrideA, 128);
-                    uint64_t d_wlo = make_smem_desc(sbase + lay.w_lo[l], kChunkStrideA, 128);
-                    for (int ks = 0; ks < nks; ++ks) {
-                        if (lane == 0) {
-                            mma_tf32_ss(tmem_base, d_whi, d_xhi, idesc, ks > 0);
-                            mma_tf32_ss(tmem_base, d_whi, d_xlo, idesc, true);
-                            mma_tf32_ss(tmem_base, d_wlo, d_xhi, idesc, true);
-                        }
-                        d_xhi += step_x; d_xlo += step_x; d_whi += step_x; d_wlo += step_x;
-                    }
-                    if (lane == 0) {
-                        mma_tf32_ss(tmem_base, make_smem_desc(sbase + lay.bias[l], kChunkStrideA, 128),
-                                    make_smem_desc(sbase + lay.ones, kChunkStrideA, 128), idesc, true);  // + bias
-                        mma_commit(bar);
+            if (l < p.L - 1) {
+                const uint32_t whi = sbase + lay.w_hi[l], wlo = sbase + lay.w_lo[l];
+                for (int h = 0; h < 2 && 64 * h < rows; ++h) {          // tile-uniform
+                    switch (np) {
+                        case 16: inner_layer<16>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        case 32: inner_layer<32>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        case 48: inner_layer<48>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        case 64: inner_layer<64>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        case 80: inner_layer<80>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        case 96: inner_layer<96>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        case 112: inner_layer<112>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
+                        default: inner_layer<128>(h, kp, a_hi, a_lo, whi, wlo, p.bias[l], p.ch[l + 1], g); break;
                     }
                 }
-                __syncwarp();
-            }
-            mbar_wait_suspend(bar, phase);
-            phase ^= 1;
-            tc_fence_after();
-
-            if (!last && lay.a_tmem && l + 2 < p.L) {
-                // the next layer is an inner one too: its A operand (K = np) goes to tensor memory
-                const uint32_t ch = kRows - 2 * np, cl = kRows - np;
-                switch (np) {
-                    case 16: mid_epilogue_tmem<16>(tmem_row, ch, cl); break;
-                    case 32: mid_epilogue_tmem<32>(tmem_row, ch, cl); break;
-                    default: mid_epilogue_tmem<48>(tmem_row, ch, cl); break;
-                }
-            } else if (!last) {
-                switch (np) {
-                    case 16: mid_epilogue<16>(tmem_row, a_hi, a_lo, r); break;
-                    case 32: mid_epilogue<32>(tmem_row, a_hi, a_lo, r); break;
-                    case 48: mid_epilogue<48>(tmem_row, a_hi, a_lo, r); break;
-                    case 64: mid_epilogue<64>(tmem_row, a_hi, a_lo, r); break;
-                    case 80: mid_epilogue<80>(tmem_row, a_hi, a_lo, r); break;
-                    case 96: mid_epilogue<96>(tmem_row, a_hi, a_lo, r); break;
-                    case 112: mid_epilogue<112>(tmem_row, a_hi, a_lo, r); break;
-                    default: mid_epilogue<128>(tmem_row, a_hi, a_lo, r); break;
-                }
-            } else if ((warp & 3) * 32 < cout_last) {
-                // ---- thread r = output channel; columns = rows of the tile, K per neighbourhood ----------
-                const bool store = r < cout_last;
-                float* ob = p.out + (static_cast<size_t>(b) * p.out_c_total + p.out_c_offset + (store ? r : 0)) * p.S + s0;
-                if (p.K == 16 || p.K == 32 || p.K == 64 || p.K == 128) {
-                    float acc = 0.f;
+            } else {
+                // D^T[channel, row] += W[channel, k] * X[row, k], one 64-channel slice at a time
+                float* ob = p.out + (static_cast<size_t>(b) * p.out_c_total + p.out_c_offset) * p.S;
+                for (int hc = 0; 64 * hc < cout_last; ++hc) {
+                    uint64_t d_whi = make_smem_desc(sbase + lay.w_hi[l] + hc * 64 * 16, kChunkStrideA);
+                    uint64_t d_wlo = make_smem_desc(sbase + lay.w_lo[l] + hc * 64 * 16, kChunkStrideA);
+                    uint64_t d_xhi = make_smem_desc(a_hi, kChunkStrideA), d_xlo = make_smem_desc(a_lo, kChunkStrideA);
+                    float acc[64];
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (32 * q < rows) {                              // tile-uniform
-                            uint32_t v[32];
-                            tmem_ld32(tmem_row + 32 * q, v);
-                            const float m_lo = relu_max16<0>(v), m_hi = relu_max16<16>(v);
-                            if (p.K == 16) {
-                                if (store) {
-                                    ob[2 * q] = m_lo;
-                                    if (2 * q + 1 < groups) ob[2 * q + 1] = m_hi;
-                                }
-                            } else {
-                                acc = max3(acc, m_lo, m_hi);
-                                const int cpn = p.K >> 5;                 // 32-column chunks per neighbourhood
-                                if (((q + 1) & (cpn - 1)) == 0) {
-                                    if (store) ob[q / cpn] = acc;
-                                    acc = 0.f;
-                                }
-                            }
-                        }
+                    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+                    fence_regs(acc);
+                    wgmma_fence();
+                    for (int ks = 0; ks < kp / 8; ++ks) {
+                        wgmma_tf32<128>(acc, d_whi, d_xhi, ks > 0);
+                        wgmma_tf32<128>(acc, d_whi, d_xlo, true);
+                        wgmma_tf32<128>(acc, d_wlo, d_xhi, true);
+                        d_xhi += desc_step(2 * kChunkStrideA); d_xlo += desc_step(2 * kChunkStrideA);
+                        d_whi += desc_step(2 * kChunkStrideA); d_wlo += desc_step(2 * kChunkStrideA);
                     }
-                } else {
-                    // any other K <= 128: running maximum over the columns, flushed every K columns
-                    float acc = 0.f;
-                    int cnt = 0, sg = 0;
-#pragma unroll 1
-                    for (int q = 0; q < 4; ++q) {
-                        if (32 * q < rows) {
-                            uint32_t v[32];
-                            tmem_ld32(tmem_row + 32 * q, v);
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) {
-                                acc = fmaxf(acc, __uint_as_float(v[i]));
-                                if (++cnt == p.K) {
-                                    if (store && sg < groups) ob[sg] = acc;
-                                    acc = 0.f; cnt = 0; ++sg;
-                                }
-                            }
-                        }
-                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(acc);
+                    store_neighbourhood_max(acc, 64 * hc + 16 * (warp & 3) + (lane >> 2), cout_last, p.bias[l], ob, p.S, s0, p.K, groups);
                 }
+                group_sync(g);             // the next tile's first-layer stores overwrite the operand these MMAs read
             }
-            tc_fence_before();             // TMEM reads done before the next layer's MMAs overwrite D
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "r"(lay.tmem_cols) : "memory");
     }
 }
 
@@ -474,21 +314,8 @@ bool make_layout(const SaParams& p, TcLayout& lay, int kGroups = kMaxGroups)
         const uint32_t wb = static_cast<uint32_t>(rows_w) * lay.kpad[l] * 4;
         lay.w_hi[l] = take(wb, 128);
         lay.w_lo[l] = take(wb, 128);
-        lay.bias[l] = take(rows_w * 32, 128);            // [rows x 8] tile: bias_hi | bias_lo | 0...
     }
-    lay.ones = take(kRows * 32, 128);
-    lay.misc = take(8 + 8 * kGroups, 16);
     lay.total = off;
-    lay.group_cols = kRows;                            // the transposed last layer fills 128 columns per group
-    lay.tmem_cols = lay.group_cols * kGroups;          // 512: all of tensor memory (one CTA per SM by design)
-    // activation operands of the inner layers in tensor memory: the accumulator (np columns from 0) and the
-    // hi / lo operands (kp columns each, at the top of the group's 128 columns) must not overlap, also with
-    // the operand the epilogue writes for the next inner layer (np columns each)
-    lay.a_tmem = (p.L >= 2 && lay.kpad[0] == 16) ? 1 : 0;
-    for (int l = 0; l + 1 < p.L && lay.a_tmem; ++l) {
-        if (lay.npad[l] + 2 * lay.kpad[l] > kRows) lay.a_tmem = 0;
-        if (l + 2 < p.L && (lay.npad[l] > 48 || 3 * lay.npad[l] > kRows)) lay.a_tmem = 0;
-    }
     lay.gpt = kRows / p.K;
     lay.tiles_per_cloud = (p.S + lay.gpt - 1) / lay.gpt;
     lay.tpc_magic = static_cast<uint32_t>(std::min<unsigned long long>((1ull << 32) / static_cast<unsigned long long>(lay.tiles_per_cloud), 0xFFFFFFFFull));
@@ -500,7 +327,7 @@ bool make_layout(const SaParams& p, TcLayout& lay, int kGroups = kMaxGroups)
 bool sa_mlp_tc_supported(const SaParams& p)
 {
     TcLayout lay{};
-    return make_layout(p, lay);
+    return make_layout(p, lay, kMaxGroups) || make_layout(p, lay, 2);
 }
 
 template <int kGroups>
@@ -508,22 +335,26 @@ int launch_tc(const SaParams& p, const TcLayout& lay, cudaStream_t st)
 {
     const int rc_attr = ensure_dynamic_smem(reinterpret_cast<const void*>(sa_mlp_tc_kernel<kGroups>), lay.total);
     if (rc_attr != TGN_OK) return rc_attr;
-    // persistent CTAs: one of 4 tile groups per SM (the whole TMEM), or two of 2 groups
+    // persistent CTAs: one of 4 tile groups per SM, or two of 2 groups
     const long long tiles = static_cast<long long>(lay.tiles_per_cloud) * p.B;
     const int grid = static_cast<int>(std::min<long long>((tiles + kGroups - 1) / kGroups, static_cast<long long>(sm_count()) * (kMaxGroups / kGroups)));
     sa_mlp_tc_kernel<kGroups><<<grid, kRows * kGroups, lay.total, st>>>(p, lay);
     return check_launch("sa_mlp_tc_kernel");
 }
 
-// groups_per_cta: 4 = one CTA owns the SM (all 64K registers, all 512 TMEM columns); 2 = half-size CTAs (32K registers, 256
-// TMEM columns) that can share an SM with the CTAs of another stream's kernels -- the host pipeline keeps the FPS of the
+// groups_per_cta: 4 = one CTA owns the SM (all 64K registers); 2 = half-size CTAs (32K registers) that can share an SM with
+// the CTAs of another stream's kernels -- the host pipeline keeps the FPS of the
 // next chunk resident, and a full-size CTA would wait for it to drain.  (Two half CTAs fit one SM only when the operand
 // tiles are small; with the bench shape the weights of the 128-row last layer make it one per SM.)
 int sa_mlp_tc_launch(SaParams p, cudaStream_t st, int groups_per_cta)
 {
     TcLayout lay{};
     if (groups_per_cta == 2 && make_layout(p, lay, 2)) return launch_tc<2>(p, lay, st);
-    if (!make_layout(p, lay, kMaxGroups)) { set_error("sa_group_mlp_max: shape not supported by the tcgen05 engine"); return TGN_ERR_INVALID; }
+    if (!make_layout(p, lay, kMaxGroups)) {
+        if (make_layout(p, lay, 2)) return launch_tc<2>(p, lay, st);       // operand tiles too large for four groups
+        set_error("sa_group_mlp_max: shape not supported by the tensor-core engine");
+        return TGN_ERR_INVALID;
+    }
     return launch_tc<kMaxGroups>(p, lay, st);
 }
 

@@ -1,21 +1,21 @@
-// sa_mlp_tcw.cu -- tcgen05 engine of the fused set-abstraction body for WIDE hidden layers (up to 128).
+// sa_mlp_tcw.cu -- warpgroup-MMA engine of the fused set-abstraction body for WIDE hidden layers (up to 128).
 //
 // The 3xTF32 engine in sa_mlp_tc.cu keeps every inter-layer operand as two tf32 tiles; at 128 channels
 // that is 128 KB per 128-row tile and nothing fits.  The reference's real pointnet_pp SA1
 // (PointNetSetAbstractionMsg(1024,[.025,.05],[32,64],6,[[128,128],[128,128]]), pointnet_pp.py:13) is
 // exactly that shape, 15x the FLOPs of the BASELINE form.  This engine keeps the same structure (tile
-// groups of 128 threads, thread = row, accumulators in TMEM, last layer transposed so that the max over
-// the K neighbours stays inside one thread) with two changes:
+// groups of 128 threads = one warpgroup, two 64-row wgmma slices per layer, accumulators in registers, last layer
+// transposed so that the max over the K neighbours stays inside one quad of threads) with two changes:
 //   * layer 0 (the raw [xyz_rel | feats] row, <= 16 channels) stays 3xTF32;
 //   * every later layer splits its operands into TWO BF16 parts, x = x1 + x2 with x1 = bf16(x) and
-//     x2 = bf16(x - x1) (16 mantissa bits kept), and issues three kind::f16 MMAs per K-step of 16
+//     x2 = bf16(x - x1) (16 mantissa bits kept), and issues three bf16 MMAs per K-step of 16
 //     (x1*w1 + x2*w1 + x1*w2) into the fp32 accumulator: ~2^-17 relative error per product -- 60x
 //     tighter than the TF32 the reference's own convolutions run in by default (SURVEY.md 7.1), inside
 //     the 1e-4 bar (measured ~1e-5 end to end), at half the operand bytes and half the MMA count of 3xTF32;
 //   * biases are added in the epilogue in fp32 (exact), not through an extra MMA.
 // Two tile groups per CTA at 128 channels (operand tile 64 KB each, 80 KB of weights), four when the layers
-// are narrow enough; persistent over tiles.  On narrow shapes the 3xTF32 engine is faster (bench shape
-// 9->[32,32,64]: 3.8 ms against 5.3 ms here) and more accurate, so the dispatcher prefers it when it fits.
+// are narrow enough; persistent over tiles.  On narrow shapes the 3xTF32 engine is more accurate, so the dispatcher
+// prefers it when it fits.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -41,7 +41,7 @@ struct WLayout {
     uint32_t act[kMaxGroups];        // per group operand buffer: [hi | lo], lo at act_lo_off
     int groups;
     uint32_t act_lo_off;
-    uint32_t misc, total;
+    uint32_t total;
     int tiles_per_cloud, gpt;
     uint32_t tpc_magic;
 };
@@ -58,45 +58,57 @@ __device__ __forceinline__ void split_bf16_pair(float a, float b, uint32_t& hi, 
     const float a1 = __uint_as_float(hi << 16), b1 = __uint_as_float(hi & 0xFFFF0000u);
     lo = pack_bf16(__fsub_rn(a, a1), __fsub_rn(b, b1));
 }
-// Inner-layer epilogue of one thread (row r): NP accumulator columns -> + bias, ReLU, bf16 hi/lo split,
-// 16-byte stores (8 K-elements each) into the next layer's K-major operand.
+// One inner layer on one 64-row slice (rows 64h..64h+63) of a group's tile -- layer 0: 3xTF32 from the tf32 hi / lo
+// operands at x_hi / a0_lo, K = 8 per MMA; later layers: three bf16 terms from x_hi / x_lo, K = 16 per MMA -- then + bias,
+// ReLU, bf16 hi/lo split and 4-byte stores of the fragment pairs into the next layer's operand (the slice only
+// overwrites its own rows, which no other slice reads).
 template <int NP>
-__device__ __forceinline__ void inner_epilogue(uint32_t tmem_row, uint32_t x_hi, uint32_t x_lo, int r, const float* __restrict__ bias,
-                                               int cout)
+__device__ __forceinline__ void inner_layer(int h, bool first, int kp, uint32_t x_hi, uint32_t x_lo, uint32_t a0_lo, uint32_t w_hi,
+                                            uint32_t w_lo, const float* __restrict__ bias, int cout, int g)
 {
+    const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+    const uint32_t lbo_w = NP * 16, row_off = h * 64 * 16;
+    uint64_t d_xh = make_smem_desc(x_hi + row_off, kChunk), d_xl = make_smem_desc((first ? a0_lo : x_lo) + row_off, kChunk);
+    uint64_t d_wh = make_smem_desc(w_hi, lbo_w), d_wl = make_smem_desc(w_lo, lbo_w);
+    float acc[NP / 2];
 #pragma unroll
-    for (int c0 = 0; c0 < NP; c0 += 32) {
-        uint32_t v[32];
-        const bool full = NP - c0 >= 32;
-        if (full) tmem_ld32(tmem_row + c0, v);
-        else tmem_ld16(tmem_row + c0, v);
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-            if (i < 16 || full) {
-                uint32_t hi[4], lo[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int c = c0 + i + 2 * u;
-                    const float b0 = c < cout ? __ldg(bias + c) : 0.f, b1 = c + 1 < cout ? __ldg(bias + c + 1) : 0.f;
-                    const float a = fmaxf(__uint_as_float(v[i + 2 * u]) + b0, 0.f);
-                    const float b = fmaxf(__uint_as_float(v[i + 2 * u + 1]) + b1, 0.f);
-                    split_bf16_pair(a, b, hi[u], lo[u]);
-                }
-                const uint32_t off = static_cast<uint32_t>((c0 + i) >> 3) * kChunk + r * 16;
-                st_shared_v4(x_hi + off, hi[0], hi[1], hi[2], hi[3]);
-                st_shared_v4(x_lo + off, lo[0], lo[1], lo[2], lo[3]);
-            }
+    for (int i = 0; i < NP / 2; ++i) acc[i] = 0.f;
+    fence_regs(acc);
+    wgmma_fence();
+    if (first) {
+        for (int ks = 0; ks < kp / 8; ++ks) {
+            wgmma_tf32<NP>(acc, d_xh, d_wh, ks > 0);
+            wgmma_tf32<NP>(acc, d_xl, d_wh, true);
+            wgmma_tf32<NP>(acc, d_xh, d_wl, true);
+            d_xh += desc_step(2 * kChunk); d_xl += desc_step(2 * kChunk); d_wh += desc_step(2 * lbo_w); d_wl += desc_step(2 * lbo_w);
+        }
+    } else {
+        for (int ks = 0; ks < kp / 16; ++ks) {
+            wgmma_bf16<NP>(acc, d_xh, d_wh, ks > 0);
+            wgmma_bf16<NP>(acc, d_xl, d_wh, true);
+            wgmma_bf16<NP>(acc, d_xh, d_wl, true);
+            d_xh += desc_step(2 * kChunk); d_xl += desc_step(2 * kChunk); d_wh += desc_step(2 * lbo_w); d_wl += desc_step(2 * lbo_w);
         }
     }
-}
-
-// max(v[B], ..., v[B+15]) with 3-input FMNMX (no ReLU here: the bias is added after the max)
-template <int B>
-__device__ __forceinline__ float max16(const uint32_t (&v)[32]) {
-    float m = fmaxf(__uint_as_float(v[B]), __uint_as_float(v[B + 1]));
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    group_sync(g);                   // every warp's MMAs have read the operand before any row of it is overwritten
+    const int row = h * 64 + w * 16 + (lane >> 2);
 #pragma unroll
-    for (int i = 2; i < 16; i += 2) m = max3(m, __uint_as_float(v[B + i]), __uint_as_float(v[B + i + 1]));
-    return m;
+    for (int i = 0; i < NP / 8; ++i) {
+        const int c = 8 * i + 2 * (lane & 3);
+        const float b0 = c < cout ? __ldg(bias + c) : 0.f, b1 = c + 1 < cout ? __ldg(bias + c + 1) : 0.f;
+        const uint32_t off = static_cast<uint32_t>(c >> 3) * kChunk + (c & 7) * 2;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            uint32_t hi, lo;
+            split_bf16_pair(fmaxf(acc[4 * i + 2 * e] + b0, 0.f), fmaxf(acc[4 * i + 2 * e + 1] + b1, 0.f), hi, lo);
+            const uint32_t o = off + (row + 8 * e) * 16;
+            st_shared_b32(x_hi + o, hi);
+            st_shared_b32(x_lo + o, lo);
+        }
+    }
 }
 
 template <int kGroups>
@@ -109,14 +121,6 @@ sa_mlp_tcw_kernel(const SaParams p, const WLayout lay)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = tid / kRows;
     const int r = tid - g * kRows;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + lay.misc);
-    const uint32_t bar = sbase + lay.misc + 8 + 8 * g;
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + lay.misc), "r"(kRows * kGroups) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (r == 0) { mbar_init(bar, 1); mbar_fence_init(); }
 
     // ---- weights, once per CTA -----------------------------------------------------------------------
     // layer 0: tf32 hi/lo B operand [np x 16] (LBO = np*16); inner layers: bf16 hi/lo B operand [np x kp]
@@ -143,14 +147,9 @@ sa_mlp_tcw_kernel(const SaParams p, const WLayout lay)
         }
     }
     proxy_fence_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot + g * kRows;
-    const uint32_t tmem_row = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
     const uint32_t x_hi = sbase + lay.act[g], x_lo = x_hi + lay.act_lo_off;
     const uint32_t a0_lo = x_hi + 4 * kChunk;       // layer 0: four tf32 chunks of hi, then four of lo
-    uint32_t phase = 0;
 
     const int cout_last = p.ch[p.L];
     const int total_tiles = lay.tiles_per_cloud * p.B;
@@ -224,112 +223,48 @@ sa_mlp_tcw_kernel(const SaParams p, const WLayout lay)
 
         for (int l = 0; l < p.L; ++l) {
             const int kp = lay.kpad[l], np = lay.npad[l];
-            const bool last = (l == p.L - 1);
             proxy_fence_async();
-            tc_fence_before();
             group_sync(g);
-            if ((warp & 3) == 0) {
-                tc_fence_after();
-                const uint64_t step = (2 * kChunk) >> 4;         // two 16-byte K-chunks of a 128-row operand per MMA
-                if (l == 0) {
-                    // D[row, n] += X0[row, k] * W0[n, k], 3xTF32, K = 8 per MMA
-                    const uint32_t idesc = make_idesc_tf32(np);
-                    const uint32_t lbo_w = static_cast<uint32_t>(np) * 16;
-                    uint64_t d_xh = make_smem_desc(x_hi, kChunk), d_xl = make_smem_desc(a0_lo, kChunk);
-                    uint64_t d_wh = make_smem_desc(sbase + lay.w_hi[0], lbo_w), d_wl = make_smem_desc(sbase + lay.w_lo[0], lbo_w);
-                    const uint64_t step_w = (2 * lbo_w) >> 4;
-                    for (int ks = 0; ks < kp / 8; ++ks) {
-                        if (lane == 0) {
-                            mma_tf32_ss(tmem_base, d_xh, d_wh, idesc, ks > 0);
-                            mma_tf32_ss(tmem_base, d_xl, d_wh, idesc, true);
-                            mma_tf32_ss(tmem_base, d_xh, d_wl, idesc, true);
-                        }
-                        d_xh += step; d_xl += step; d_wh += step_w; d_wl += step_w;
-                    }
-                } else if (!last) {
-                    // D[row, n] += X[row, k] * W[n, k], three bf16 terms, K = 16 per MMA
-                    const uint32_t idesc = make_idesc_bf16(np);
-                    const uint32_t lbo_w = static_cast<uint32_t>(np) * 16;
-                    uint64_t d_xh = make_smem_desc(x_hi, kChunk), d_xl = make_smem_desc(x_lo, kChunk);
-                    uint64_t d_wh = make_smem_desc(sbase + lay.w_hi[l], lbo_w), d_wl = make_smem_desc(sbase + lay.w_lo[l], lbo_w);
-                    const uint64_t step_w = (2 * lbo_w) >> 4;
-                    for (int ks = 0; ks < kp / 16; ++ks) {
-                        if (lane == 0) {
-                            mma_bf16_ss(tmem_base, d_xh, d_wh, idesc, ks > 0);
-                            mma_bf16_ss(tmem_base, d_xl, d_wh, idesc, true);
-                            mma_bf16_ss(tmem_base, d_xh, d_wl, idesc, true);
-                        }
-                        d_xh += step; d_xl += step; d_wh += step_w; d_wl += step_w;
-                    }
-                } else {
-                    // D^T[channel, row] += W[channel, k] * X[row, k], three bf16 terms
-                    const uint32_t idesc = make_idesc_bf16(kRows);
-                    uint64_t d_xh = make_smem_desc(x_hi, kChunk), d_xl = make_smem_desc(x_lo, kChunk);
-                    uint64_t d_wh = make_smem_desc(sbase + lay.w_hi[l], kChunk), d_wl = make_smem_desc(sbase + lay.w_lo[l], kChunk);
-                    for (int ks = 0; ks < kp / 16; ++ks) {
-                        if (lane == 0) {
-                            mma_bf16_ss(tmem_base, d_wh, d_xh, idesc, ks > 0);
-                            mma_bf16_ss(tmem_base, d_wh, d_xl, idesc, true);
-                            mma_bf16_ss(tmem_base, d_wl, d_xh, idesc, true);
-                        }
-                        d_xh += step; d_xl += step; d_wh += step; d_wl += step;
+            if (l < p.L - 1) {
+                const uint32_t wh = sbase + lay.w_hi[l], wl = sbase + lay.w_lo[l];
+                for (int h = 0; h < 2 && 64 * h < rows; ++h) {          // tile-uniform
+                    switch (np) {
+                        case 16: inner_layer<16>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        case 32: inner_layer<32>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        case 48: inner_layer<48>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        case 64: inner_layer<64>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        case 80: inner_layer<80>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        case 96: inner_layer<96>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        case 112: inner_layer<112>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
+                        default: inner_layer<128>(h, l == 0, kp, x_hi, x_lo, a0_lo, wh, wl, p.bias[l], p.ch[l + 1], g); break;
                     }
                 }
-                if (lane == 0) mma_commit(bar);
-                __syncwarp();
-            }
-            mbar_wait_suspend(bar, phase);
-            phase ^= 1;
-            tc_fence_after();
-
-            if (!last) {
-                switch (np) {
-                    case 16: inner_epilogue<16>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    case 32: inner_epilogue<32>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    case 48: inner_epilogue<48>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    case 64: inner_epilogue<64>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    case 80: inner_epilogue<80>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    case 96: inner_epilogue<96>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    case 112: inner_epilogue<112>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                    default: inner_epilogue<128>(tmem_row, x_hi, x_lo, r, p.bias[l], p.ch[l + 1]); break;
-                }
-            } else if ((warp & 3) * 32 < cout_last) {
-                // thread r = output channel; columns = rows of the tile; max over the K columns of a neighbourhood,
-                // then + bias and ReLU (both monotone, so they commute with the max)
-                const bool store = r < cout_last;
-                const float bv = store ? __ldg(p.bias[l] + r) : 0.f;
-                float* ob = p.out + (static_cast<size_t>(b) * p.out_c_total + p.out_c_offset + (store ? r : 0)) * p.S + s0;
-                float acc = -INFINITY;
+            } else {
+                // D^T[channel, row] += W[channel, k] * X[row, k], three bf16 terms, one 64-channel slice at a time
+                float* ob = p.out + (static_cast<size_t>(b) * p.out_c_total + p.out_c_offset) * p.S;
+                for (int hc = 0; 64 * hc < cout_last; ++hc) {
+                    uint64_t d_wh = make_smem_desc(sbase + lay.w_hi[l] + hc * 64 * 16, kChunk);
+                    uint64_t d_wl = make_smem_desc(sbase + lay.w_lo[l] + hc * 64 * 16, kChunk);
+                    uint64_t d_xh = make_smem_desc(x_hi, kChunk), d_xl = make_smem_desc(x_lo, kChunk);
+                    float acc[64];
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    if (32 * q < rows) {                              // tile-uniform
-                        uint32_t v[32];
-                        tmem_ld32(tmem_row + 32 * q, v);
-                        const float m_lo = max16<0>(v), m_hi = max16<16>(v);
-                        if (p.K == 16) {
-                            if (store) {
-                                ob[2 * q] = fmaxf(m_lo + bv, 0.f);
-                                if (2 * q + 1 < groups) ob[2 * q + 1] = fmaxf(m_hi + bv, 0.f);
-                            }
-                        } else {
-                            acc = max3(acc, m_lo, m_hi);
-                            const int cpn = p.K >> 5;
-                            if (((q + 1) & (cpn - 1)) == 0) {
-                                if (store) ob[q / cpn] = fmaxf(acc + bv, 0.f);
-                                acc = -INFINITY;
-                            }
-                        }
+                    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+                    fence_regs(acc);
+                    wgmma_fence();
+                    for (int ks = 0; ks < kp / 16; ++ks) {
+                        wgmma_bf16<128>(acc, d_wh, d_xh, ks > 0);
+                        wgmma_bf16<128>(acc, d_wh, d_xl, true);
+                        wgmma_bf16<128>(acc, d_wl, d_xh, true);
+                        d_xh += desc_step(2 * kChunk); d_xl += desc_step(2 * kChunk); d_wh += desc_step(2 * kChunk); d_wl += desc_step(2 * kChunk);
                     }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(acc);
+                    store_neighbourhood_max(acc, 64 * hc + 16 * (warp & 3) + (lane >> 2), cout_last, p.bias[l], ob, p.S, s0, p.K, groups);
                 }
+                group_sync(g);             // the next tile's first-layer stores overwrite the operand these MMAs read
             }
-            tc_fence_before();
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "r"(kRows * kGroups) : "memory");
     }
 }
 
@@ -363,7 +298,6 @@ bool make_wlayout_groups(const SaParams& p, WLayout& lay, int kGroups)
         lay.w_hi[l] = take(wb, 128);
         lay.w_lo[l] = take(wb, 128);
     }
-    lay.misc = take(8 + 8 * kGroups, 16);
     lay.total = off;
     lay.gpt = kRows / p.K;
     lay.tiles_per_cloud = (p.S + lay.gpt - 1) / lay.gpt;
@@ -399,7 +333,7 @@ bool sa_mlp_tcw_supported(const SaParams& p)
 int sa_mlp_tcw_launch(SaParams p, cudaStream_t st)
 {
     WLayout lay{};
-    if (!make_wlayout(p, lay)) { set_error("sa_group_mlp_max: shape not supported by the wide tcgen05 engine"); return TGN_ERR_INVALID; }
+    if (!make_wlayout(p, lay)) { set_error("sa_group_mlp_max: shape not supported by the wide tensor-core engine"); return TGN_ERR_INVALID; }
     return lay.groups == 4 ? launch_tcw<4>(p, lay, st) : launch_tcw<2>(p, lay, st);
 }
 

@@ -5,7 +5,7 @@ batch that lives in pinned host memory can be processed in chunks: the H2D copie
 queued back to back on a copy stream, groups of chunks compute on one of a few compute streams as
 soon as they have landed, and results return on a third stream (PCIe is full duplex).
 
-    pipe = HostPipeline(sa_module, chunk_clouds=148, n_streams=2)
+    pipe = HostPipeline(sa_module, chunk_clouds=132, n_streams=2)
     pipe(host_feats, out_xyz_host, out_points_host)      # all pinned; returns after a full sync
 
 For a STREAM of batches (a loader handing over one pinned batch after another) the copies of batch i+1 need not wait for batch i:
@@ -33,14 +33,11 @@ class HostPipeline:
     """H2D copies run back to back on a dedicated stream in chunks of ``chunk_clouds`` into ONE device
     buffer; compute runs on ``n_streams`` streams over GROUPS of consecutive chunks (``groups``: chunks
     per group in order, the last but one repeating, the last entry being the size of the final group) as soon as the last chunk of a group has landed;
-    results return on a third stream.  Measured on B200 (1184 clouds of 24k points, profiles/r2_summary.md): the kernels of
-    a chunk are sized to own an SM (the group-MLP CTA takes all 64K registers and all 512 TMEM columns, the FPS sort
-    prologue 192 KB of shared memory), so chunks on different streams mostly run one after the other and the end-to-end
-    time is  first H2D + chunks x (compute time of one chunk): 1.55 ms + 8 x 2.07 ms with 148-cloud chunks, against
-    12.4 ms of PCIe transfer.  One chunk per group is best; what moved the number in round 2 was the small-batch FPS
-    (1.67 -> 1.07 ms per 148 clouds), not more streams."""
+    results return on a third stream.  The kernels of a chunk are sized to own an SM (the group-MLP CTA takes all 64K
+    registers, the FPS sort prologue most of the shared memory), so chunks on different streams mostly run one after the
+    other and the end-to-end time is about first H2D + chunks x (compute time of one chunk)."""
 
-    def __init__(self, module: torch.nn.Module, chunk_clouds: int = 148, n_streams: int = 2,
+    def __init__(self, module: torch.nn.Module, chunk_clouds: int = 132, n_streams: int = 2,
                  groups: Sequence[int] = (1,), fps_mode: int = None, sa_engine: int = None):
         self.module = module
         self.chunk = int(chunk_clouds)

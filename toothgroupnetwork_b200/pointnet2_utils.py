@@ -6,11 +6,11 @@ Same public names, signatures, tensor layouts ((B,C,N) channel-first in and out)
 reference, so ``models/modules/{pointnet_pp,tsg_centroid_module,tsg_seg_module}.py`` and the
 losses import it unchanged and checkpoints load.  What changes is underneath:
 
-* FPS, ball query, 3-NN, gathers and transposes are hand-written sm_100a kernels (the reference
+* FPS, ball query, 3-NN, gathers and transposes are hand-written sm_90a kernels (the reference
   runs ball query / 3-NN as dense torch ops with (S,N) matrices and full sorts);
 * in inference (``module.eval()`` and no autograd) a set-abstraction level is ONE fused kernel
   per radius branch: gather -> [xyz_rel|feats] -> (conv1x1+BN+ReLU)* -> max over K, BatchNorm
-  folded into the conv weights, nothing materialised (tcgen05 3xTF32 engine, fp32 engine as
+  folded into the conv weights, nothing materialised (wgmma 3xTF32 engine, fp32 engine as
   fallback);
 * when BatchNorm must use batch statistics (``module.training``) or gradients are needed, the
   grouped tensor is built by the CUDA gather (with its scatter-add backward) and the 1x1
@@ -35,12 +35,13 @@ from . import pointops
 
 SA_FUSED_MAX_WIDTH = 128
 SA_FUSED_MAX_LAYERS = 4
-ENGINE_AUTO, ENGINE_FP32, ENGINE_TC, ENGINE_TCW, ENGINE_TC8, ENGINE_TC_HALF = 0, 1, 2, 3, 4, 5     # TCW: wide layers (bf16x2); TC8: eight tile groups, bf16x3; TC_HALF: engine 2 in half-size CTAs
+ENGINE_AUTO, ENGINE_FP32, ENGINE_TC, ENGINE_TCW, ENGINE_TC_HALF = 0, 1, 2, 3, 5     # TCW: wide layers (bf16x2); TC_HALF: engine 2 in half-size CTAs
 _sa_engine = ENGINE_AUTO
 
 
 def set_sa_engine(engine: int) -> None:
-    """Select the engine of the fused set-abstraction kernel (0 auto, 1 fp32 CUDA cores, 2 tcgen05)."""
+    """Select the engine of the fused set-abstraction kernel (0 auto, 1 fp32 CUDA cores, 2 3xTF32 tensor cores, 3 wide
+    bf16x2 tensor cores, 5 engine 2 in half-size CTAs)."""
     global _sa_engine
     _sa_engine = int(engine)
 
@@ -211,8 +212,8 @@ def set_ball_path(path: int) -> None:
 
 
 # ---- which torch arithmetic the neighbourhood searches reproduce ---------------------------------------------------
-# square_distance (:38-40) adds torch.sum(p ** 2, -1) of both operands.  Measured on B200 / torch 2.11
-# (scripts/diag_sumsq.py, profiles/r2_parity.md): on CUDA that sum rounds as (x*x + z*z) + y*y when the (..., 3) operand is
+# square_distance (:38-40) adds torch.sum(p ** 2, -1) of both operands.  Measured with torch 2.11
+# (scripts/diag_sumsq.py): on CUDA that sum rounds as (x*x + z*z) + y*y when the (..., 3) operand is
 # CONTIGUOUS (vectorised reduce) and as (x*x + y*y) + z*z when it is a strided view -- and always the latter on the CPU.
 # The reference's modules mix both: new_xyz fresh out of index_points is contiguous, xyz.permute(0, 2, 1) of the raw
 # input is a view, the (B,3,S) coordinates a set-abstraction level returns are views that turn contiguous again when
@@ -392,7 +393,7 @@ SA_FUSED_AUTO_MAX_WIDTH = 64      # widest layer of the 3xTF32 single-kernel eng
 
 def fused_supported(channels: Sequence[int]) -> bool:
     """Shapes the single-kernel (eval-mode BatchNorm) engines take.  On the automatic path only the fp32-grade
-    ones are used (3xTF32 tcgen05 up to 64 channels, else the layer-per-launch chain of csrc/pw_mlp.cu with
+    ones are used (3xTF32 tensor cores up to 64 channels, else the layer-per-launch chain of csrc/pw_mlp.cu with
     three-part operands): the wide bf16x2 engine (ENGINE_TCW, ~1e-5 norm-wise) misses the ELEMENT-WISE 1e-4 bound on
     small activations (measured 4e-4 at a 1 % floor, tests/test_gpu_reference_live.py) and is kept for explicit use."""
     widest = SA_FUSED_MAX_WIDTH if _sa_engine != ENGINE_AUTO else SA_FUSED_AUTO_MAX_WIDTH
@@ -415,7 +416,7 @@ def sa_group_mlp_max(xyz_t, feats_t, new_xyz_t, group_idx, xyz_first: bool, fold
 
 # ------------------------------------------------------------------------------------------ conv1x1 + BatchNorm chains (any width, any BN mode)
 class _PwChain:
-    """Launch plan of a [conv1x1 -> BatchNorm -> ReLU]* chain on the tcgen05 layer kernel (csrc/pw_mlp.cu):
+    """Launch plan of a [conv1x1 -> BatchNorm -> ReLU]* chain on the tensor-core layer kernel (csrc/pw_mlp.cu):
     one launch per layer, BatchNorm of layer l applied while layer l+1 builds its operand, batch statistics
     (training mode -- what every reference call site runs, inference included) accumulated in fp64 by the
     producing launch, running statistics updated in-kernel like torch does.  Packed bf16 hi/lo weights are
@@ -614,7 +615,7 @@ class PointNetSetAbstraction(nn.Module):
         return (not any(b.training for b in self.mlp_bns)) and fused_supported(chans) and not _wants_grad(self, xyz, points)
 
     def _pw_ok(self, xyz, points) -> bool:
-        """Layer-per-launch tcgen05 chain: any width, batch-statistics or running-statistics BatchNorm, no autograd."""
+        """Layer-per-launch tensor-core chain: any width, batch-statistics or running-statistics BatchNorm, no autograd."""
         return _pw_enabled and _PwChain.supported(self.mlp_convs, self.mlp_bns) and not _wants_grad(self, xyz, points)
 
     def forward(self, xyz, points):
@@ -754,7 +755,7 @@ class PointNetFeaturePropagation(nn.Module):
         S = x2.shape[1]
         if (_pw_enabled and _PwChain.supported(self.mlp_convs, self.mlp_bns)
                 and not _wants_grad(self, xyz1, xyz2, points1, points2)):
-            # tcgen05 chain: layer 0 reads [points1 (channel-first) | interpolated (point-major)] in place
+            # tensor-core chain: layer 0 reads [points1 (channel-first) | interpolated (point-major)] in place
             if S == 1:
                 interp, strides = p2, (p2.shape[2], 0, 1)                      # (B,1,D2): every fine point gets the one coarse row
             else:

@@ -3,7 +3,7 @@
 Same public names, positional signatures, dtypes and layouts as the reference (packed
 ``(n_total, C)`` tensors with cumulative int32 ``offset``; see SURVEY.md 8b), so the callers in
 ``models/modules/cbl_point_transformer/{blocks,heads,basic_operators}.py`` and ``gen_utils.fps``
-run unchanged.  Every op launches hand-written sm_100a kernels on the current stream; there is
+run unchanged.  Every op launches hand-written sm_90a kernels on the current stream; there is
 no CPU path.  Reference line numbers below refer to that file.
 """
 from __future__ import annotations
