@@ -105,6 +105,16 @@ size_t tgn_dbscan_bytes(int n);
 int tgn_dbscan(int n, const float *xyz, double eps, int min_samples, void *workspace, int *labels, unsigned char *core, int *n_clusters,
                void *stream);
 
+/* Exact float64 kNN with a fused label vote: the answer of sklearn KDTree(xyz).query(queries, k) -- boundary detection of
+ * InferencePipeLine.get_boundary_sampled_feats (inference_pipeline_tgn.py:289-330).  xyz (n,3) and queries (m,3) float64
+ * DEVICE; 1 <= k <= 64, k <= n.  Distances d2 = (dx*dx + dy*dy) + dz*dz in float64 without contraction, neighbours ascending
+ * by (d2, index).  Each call builds a uniform grid into a DEVICE workspace of tgn_knn_f64_bytes(n) bytes and queries it.
+ * Outputs, each optional (NULL): idx (m,k) int64; dist (m,k) float64 = correctly rounded sqrt(d2); nn0 (m) int32 = index of
+ * the nearest point; agree (m) int32 = how many of the k neighbours carry labels[nn0] (needs labels (n) int32). */
+size_t tgn_knn_f64_bytes(int n);
+int tgn_knn_f64(int n, int m, int k, const double *xyz, const double *queries, void *workspace, const int *labels, long long *idx,
+                double *dist, int *nn0, int *agree, void *stream);
+
 /* kNN through a per-segment uniform grid: identical answers to tgn_knnquery (distinct distances: order-independent;
  * ties among the k+1 best: the query is re-run with the reference's index-order heap), ~100x fewer distance evaluations
  * on 24k-point clouds.  The grid depends only on (xyz, offset): build it once into a caller-owned DEVICE workspace of

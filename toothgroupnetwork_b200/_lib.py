@@ -24,6 +24,7 @@ _SIGS = {
     "tgn_crop_knn": [_i, _i, _i, _i, _vp, _vp, _vp, _i, _vp],
     "tgn_pt_layer_set_cta_threshold": [_i],
     "tgn_dbscan": [_i, _vp, ctypes.c_double, _i, _vp, _vp, _vp, _vp, _vp],
+    "tgn_knn_f64": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_csr_build": [ctypes.c_longlong, _i, _vp, _vp, _vp],
     "tgn_gather_backward_det": [ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp],
     "tgn_weighted_gather_backward_det": [ctypes.c_longlong, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],
@@ -108,7 +109,7 @@ REFERENCE_LAUNCHERS = [
     "subtraction_forward_cuda_launcher", "subtraction_backward_cuda_launcher",
     "aggregation_forward_cuda_launcher", "aggregation_backward_cuda_launcher",
 ]
-EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes"]
+EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes"]
 
 
 class TgnError(RuntimeError):
@@ -140,6 +141,8 @@ def load() -> ctypes.CDLL:
     lib.tgn_knn_grid_bytes.restype = ctypes.c_size_t
     lib.tgn_dbscan_bytes.argtypes = [_i]
     lib.tgn_dbscan_bytes.restype = ctypes.c_size_t
+    lib.tgn_knn_f64_bytes.argtypes = [_i]
+    lib.tgn_knn_f64_bytes.restype = ctypes.c_size_t
     lib.tgn_pw_struct_size.argtypes = [_i]
     lib.tgn_pw_struct_size.restype = _i
     lib.tgn_pt_layer_struct_size.restype = _i

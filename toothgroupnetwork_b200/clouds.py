@@ -49,6 +49,23 @@ def arch_features(n: int, seed: int = 0) -> torch.Tensor:
     return torch.cat([xyz, normal], 1).t().contiguous().unsqueeze(0)
 
 
+def boundary_inputs(m: int, seed: int = 0, n_sampled: int = 24000, label_noise: float = 0.0):
+    """numpy inputs of the boundary resampling between tgnet's two networks (inference_pipeline_tgn.py:289-330):
+    org_feats (m,6) float64 -- dental_arch vertices with float64 jitter (coordinates that are not float32 values, so distances do
+    not tie) and their normals; sampled_feats (n_sampled,6) -- a seeded subset of those rows, as the FPS of the mesh would be;
+    point_labels (n_sampled,) float64 -- the arch's tooth bins + 1 (0 = gingiva), a share ``label_noise`` of them replaced by
+    random labels (a poorly trained first network)."""
+    import numpy as np
+    xyz, normal, label = dental_arch(m, seed)
+    rng = np.random.default_rng(int(seed) + 104729)
+    org = np.concatenate([xyz.double().numpy() + rng.normal(0.0, 1e-4, (m, 3)), normal.double().numpy()], 1)
+    rows = np.sort(rng.choice(m, n_sampled, replace=False))
+    labels = label.numpy()[rows].astype(np.float64) + 1.0
+    noisy = rng.random(n_sampled) < label_noise
+    labels[noisy] = rng.integers(0, 17, int(noisy.sum())).astype(np.float64)
+    return org, org[rows].copy(), labels
+
+
 def with_duplicates(xyz: torch.Tensor, seed: int = 0) -> torch.Tensor:
     """Every vertex twice, shuffled: the FPS / kNN tie-break stress input (SURVEY.md 7.1)."""
     g = torch.Generator().manual_seed(int(seed) + 7919)

@@ -77,6 +77,17 @@ def accelerate_blocks(blocks_module=None) -> None:
     blocks_fused.accelerate(blocks_module)
 
 
+def accelerate_inference_pipeline(module=None) -> None:
+    """Optional: run the boundary detection and resampling between the two networks of a tgnet inference
+    (``InferencePipeLine.get_boundary_sampled_feats``, inference_pipelines/inference_pipeline_tgn.py:289-330: float64 KDTree kNN,
+    label vote, random boundary subset, FPS) on the GPU through ``toothgroupnetwork_b200.boundary``.  Imports
+    ``inference_pipelines.inference_pipeline_tgn`` from ``sys.path`` when no module is passed."""
+    from . import boundary
+    if module is None:
+        module = importlib.import_module("inference_pipelines.inference_pipeline_tgn")
+    boundary.accelerate(module)
+
+
 def uninstall() -> None:
     for alias in _TARGETS:
         sys.modules.pop(alias, None)
