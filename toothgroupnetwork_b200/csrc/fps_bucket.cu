@@ -6,10 +6,11 @@
 //
 //  * prologue kernel (one CTA per cloud): the cloud is sorted by a Morton code (stable LSD radix sort;
 //    clouds up to 26.6k points entirely in shared memory on 17-bit codes, larger ones through global
-//    memory on 21-bit codes) so that every 64 consecutive points -- a BUCKET, two points per lane of
-//    a warp -- are spatial neighbours; each bucket gets an axis-aligned bounding box (inflated by an
-//    absolute slack).  Sorted points are stored lane-major as pairs, (x0,x1,y0,y1) and
-//    (z0,z1,key0,key1), so that the distance update runs on the packed fp32x2 pipe.
+//    memory on 21-bit codes) so that every 64 consecutive points -- a BUCKET, two adjacent points per
+//    lane of a warp -- are spatial neighbours; each bucket gets an axis-aligned bounding box (inflated
+//    by an absolute slack).  Sorted points are stored lane-major as 16-byte pairs, (x0,x1,y0,y1) and
+//    (z0,z1,t0,t1), so that the distance update runs on the packed fp32x2 pipe; their tie keys live
+//    in an array of their own that the update loop does not read.
 //  * main kernel (one CTA of 4, 8 or 16 warps per cloud, 8, 4 or 2 CTAs per SM); warp w OWNS the
 //    contiguous bucket range [w*R, (w+1)*R) and caches its best candidate and the union box of the
 //    range.  Per iteration, with o the new sample:
@@ -20,15 +21,17 @@
 //      (b) surviving buckets are spread over all warps, one warp per bucket, two buckets in flight: the
 //          64 points are re-evaluated with the reference's exact arithmetic (FMUL dy*dy,
 //          FFMA dx*dx+., FFMA dz*dz+., FMNMX; the packed forms round each half identically),
-//          changed minima are written back and the bucket's cached candidate (max t, tie key,
+//          changed minima are written back and the bucket's cached candidate (max t, sorted position,
 //          coordinates) is refreshed;
 //      (c) owner warps whose range was touched refresh their range candidate; the block arg-max is
 //          one CREDUX pair over the range candidates.
-//    Ties are resolved by the reference's order (bitrev(j mod BS), j div BS) on ORIGINAL indices:
-//    that key travels with each sorted point (j is recovered from it), so the result does not depend
-//    on the internal order.
-//  * the bucket table lives in shared memory (52 B per bucket), the points in L2/HBM (20 B/point); an
-//    iteration is three block barriers and one memory round trip, hidden by the other CTAs of the SM.
+//    Ties are resolved by the reference's order (bitrev(j mod BS), j div BS) on ORIGINAL indices, so the
+//    result does not depend on the internal order.  Candidates carry their sorted position; a reduction
+//    reads the keys of the tied entries only when more than one entry holds the maximum.  The loop
+//    records sorted positions in idx and maps them to original indices in one pass at the end.
+//  * the bucket table lives in shared memory (52 B per bucket), the points in L2/HBM (16 B/point read per
+//    visit, 4 B/point of keys apart); an iteration is three block barriers and one
+//    memory round trip, hidden by the other CTAs of the SM.
 #include <algorithm>
 #include <climits>
 
@@ -50,14 +53,14 @@ constexpr int kMaxBuckets = 3600;   // 52 B of shared memory per bucket
 constexpr unsigned FULL = 0xffffffffu;
 
 struct BucketWs {
-    float4* pa;       // [b][stride/2]  bucket-major, lane-major pairs (x0, x1, y0, y1); point 1 is 32 places after point 0
-    float4* pb;       // [b][stride/2]  (z0, z1, bits(key0), bits(key1)); pads carry key INT_MAX
-    float2* tv;       // [b][stride/2]  running minima (t0, t1); pads -1
+    float4* pa;       // [b][stride/2]  bucket-major, lane-major pairs (x0, x1, y0, y1); lane l holds sorted points 2l, 2l+1
+    float4* pb;       // [b][stride/2]  (z0, z1, t0, t1): coordinates and running minima; pads carry t = -1
+    int2* keys;       // [b][stride/2]  tie keys (key0, key1) of the same pairs; pads INT_MAX
     uint2* key_a;     // [b][stride]    radix ping (clouds too large for the shared-memory sort)
     uint2* key_b;     // [b][stride]    radix pong
     float4* box_lo;   // [b][nbmax]     inflated box minimum, w = initial max t of the bucket
     float4* box_hi;   // [b][nbmax]     inflated box maximum, w = bits of that max t
-    float4* bxyz;     // [b][nbmax]     initial cached candidate (x, y, z, bits(key))
+    float4* bxyz;     // [b][nbmax]     initial cached candidate (x, y, z, bits(sorted position in the cloud))
     int stride;       // points per cloud slot (multiple of 64)
     int nbmax;        // buckets per cloud slot
 };
@@ -82,6 +85,55 @@ __device__ __forceinline__ float box_dist2(float lx, float ly, float lz, float h
     const float ey = fmaxf(fmaxf(ly - oy, oy - hy), 0.f);
     const float ez = fmaxf(fmaxf(lz - oz, oz - hz), 0.f);
     return ex * ex + ey * ey + ez * ez;
+}
+// Tie key of the point at sorted position p of this cloud (p < 0: no point, sorts last).
+__device__ __forceinline__ int key_at(const int* __restrict__ key, int p) { return p < 0 ? INT_MAX : __ldg(key + p); }
+// Lane holding the warp's best (v, p): larger value bits, then the smaller tie key of sorted position p.  The keys are read only
+// when more than one lane holds the maximum.
+__device__ __forceinline__ int warp_best_lane(int v, int p, const int* __restrict__ key, int& wv) {
+    wv = __reduce_max_sync(FULL, v);
+    const unsigned tied = __ballot_sync(FULL, v == wv);
+    if (__popc(tied) == 1) return __ffs(tied) - 1;
+    const int k = v == wv ? key_at(key, p) : INT_MAX;
+    const int wk = __reduce_min_sync(FULL, k);
+    return __ffs(__ballot_sync(FULL, v == wv && k == wk)) - 1;
+}
+// Candidate of a bucket from its 64 minima (n0, n1 of lane l = sorted points 2l, 2l+1): returns the lane holding it, its value
+// bits in wmax and, in take1, whether each lane's better point is its second one.  kp = the lane's pair of tie keys, read only
+// on a tie.
+__device__ __forceinline__ int bucket_best(float n0, float n1, const int2* kp, int& wmax, bool& take1) {
+    const int b0 = __float_as_int(n0), b1 = __float_as_int(n1);          // pads stay at -1
+    take1 = b1 > b0;
+    const int bl = take1 ? b1 : b0;
+    wmax = __reduce_max_sync(FULL, bl);
+    const unsigned tied = __ballot_sync(FULL, bl == wmax);
+    const unsigned pair = __ballot_sync(FULL, bl == wmax && b0 == b1);
+    if (__popc(tied) == 1 && pair == 0u) return __ffs(tied) - 1;
+    int kl = INT_MAX;
+    if (bl == wmax) {
+        const int2 k = __ldg(kp);
+        if (b0 == b1) take1 = k.y < k.x;
+        kl = take1 ? k.y : k.x;
+    }
+    const int wk = __reduce_min_sync(FULL, kl);
+    return __ffs(__ballot_sync(FULL, bl == wmax && kl == wk)) - 1;
+}
+// Sorted positions in idx[1, m) -> original indices (start_n + j), after the sampling loop.
+__device__ __forceinline__ void positions_to_indices(int* idx, int m, int start_n, const int* __restrict__ key, int bs_log2,
+                                                     int tid, int nthreads) {
+    __syncthreads();
+    for (int i = 1 + tid; i < m; i += nthreads) idx[i] = start_n + key_to_index(__ldg(key + idx[i]), bs_log2);
+}
+// Final running minima -> tmp (original order).
+__device__ __forceinline__ void write_tmp(float* tmp, int start_n, int nb, const float4* pb, const int2* __restrict__ keys,
+                                          int bs_log2, int tid, int nthreads) {
+    __syncthreads();
+    for (int q = tid; q < nb * 32; q += nthreads) {           // q = bucket * 32 + lane
+        const float4 B = __ldcg(pb + q);
+        const int2 k = __ldg(keys + q);
+        if (k.x != INT_MAX) tmp[start_n + key_to_index(k.x, bs_log2)] = B.z;
+        if (k.y != INT_MAX) tmp[start_n + key_to_index(k.y, bs_log2)] = B.w;
+    }
 }
 __device__ __forceinline__ unsigned spread3(unsigned x) {   // 10 bits -> every third bit
     x = (x | (x << 16)) & 0x030000FFu;
@@ -232,7 +284,7 @@ fps_bucket_sort_kernel(const float* __restrict__ xyz, const int* __restrict__ of
     const float* cx = xyz + 3 * static_cast<size_t>(start_n);
     float4* __restrict__ pa = ws.pa + static_cast<size_t>(cloud) * (ws.stride / 2);
     float4* __restrict__ pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
-    float2* __restrict__ tv2 = ws.tv + static_cast<size_t>(cloud) * (ws.stride / 2);
+    int2* __restrict__ keys = ws.keys + static_cast<size_t>(cloud) * (ws.stride / 2);
     uint2* ka = SMEM_ ? nullptr : ws.key_a + static_cast<size_t>(cloud) * ws.stride;
     uint2* kb = SMEM_ ? nullptr : ws.key_b + static_cast<size_t>(cloud) * ws.stride;
 
@@ -294,8 +346,8 @@ fps_bucket_sort_kernel(const float* __restrict__ xyz, const int* __restrict__ of
     }
 
     // ---- sorted points, running minima, bucket boxes and initial candidates -------------------------------
-    // A warp writes one bucket (64 consecutive sorted points, two per lane) per step and reduces its box
-    // and best candidate from the registers it just filled; kGatherUnroll buckets are in flight per warp.
+    // A warp writes one bucket (64 consecutive sorted points, two adjacent ones per lane) per step and reduces its
+    // box and best candidate from the registers it just filled; kGatherUnroll buckets are in flight per warp.
     const int nb = (n + kBP - 1) / kBP;
     float4* __restrict__ blo = ws.box_lo + static_cast<size_t>(cloud) * ws.nbmax;
     float4* __restrict__ bhi = ws.box_hi + static_cast<size_t>(cloud) * ws.nbmax;
@@ -307,7 +359,7 @@ fps_bucket_sort_kernel(const float* __restrict__ xyz, const int* __restrict__ of
         for (int u = 0; u < kGatherUnroll; ++u)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int p = (bk0 + u * kNW) * kBP + 32 * h + lane;
+                const int p = (bk0 + u * kNW) * kBP + 2 * lane + h;
                 j[u][h] = p < n ? (SMEM_ ? static_cast<int>(sb[p] & 0x7FFFu) : static_cast<int>(kb[p].y)) : -1;
             }
 #pragma unroll
@@ -330,8 +382,8 @@ fps_bucket_sort_kernel(const float* __restrict__ xyz, const int* __restrict__ of
             const int k0 = j[u][0] >= 0 ? point_key(j[u][0], bs_log2) : INT_MAX;
             const int k1 = j[u][1] >= 0 ? point_key(j[u][1], bs_log2) : INT_MAX;
             pa[bk * 32 + lane] = make_float4(x[u][0], x[u][1], y[u][0], y[u][1]);
-            pb[bk * 32 + lane] = make_float4(z[u][0], z[u][1], __int_as_float(k0), __int_as_float(k1));
-            tv2[bk * 32 + lane] = make_float2(t[u][0], t[u][1]);
+            pb[bk * 32 + lane] = make_float4(z[u][0], z[u][1], t[u][0], t[u][1]);
+            keys[bk * 32 + lane] = make_int2(k0, k1);
             const bool ok0 = j[u][0] >= 0, ok1 = j[u][1] >= 0;
             const float lx = ordered_min(fminf(ok0 ? x[u][0] : INFINITY, ok1 ? x[u][1] : INFINITY));
             const float ly = ordered_min(fminf(ok0 ? y[u][0] : INFINITY, ok1 ? y[u][1] : INFINITY));
@@ -350,7 +402,7 @@ fps_bucket_sort_kernel(const float* __restrict__ xyz, const int* __restrict__ of
             }
             if (bl == wmax && kl == wkey)
                 bxyz[bk] = make_float4(take1 ? x[u][1] : x[u][0], take1 ? y[u][1] : y[u][0], take1 ? z[u][1] : z[u][0],
-                                       __int_as_float(wkey));
+                                       __int_as_float(bk * kBP + 2 * lane + (take1 ? 1 : 0)));
         }
     }
 }
@@ -368,7 +420,7 @@ fps_bucket_kernel(const float* __restrict__ xyz, const int* __restrict__ offset,
     constexpr int kMT = MT_, kMNW = MT_ / 32;     // shadow the defaults
     extern __shared__ __align__(16) unsigned char dyn[];
     __shared__ int nact;
-    __shared__ int4 wres[kMNW];           // per owner warp: (value bits, key, bucket, -)
+    __shared__ int4 wres[kMNW];           // per owner warp: (value bits, sorted position, bucket, -)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cloud = blockIdx.x;
@@ -383,12 +435,13 @@ fps_bucket_kernel(const float* __restrict__ xyz, const int* __restrict__ offset,
     const int nb = (n + kBP - 1) / kBP;
     float4* blo = reinterpret_cast<float4*>(dyn);                                   // [nbmax] box min, w = skip threshold
     float4* bhi = blo + ws.nbmax;                                                   // [nbmax] box max, w = candidate value bits
-    float4* cxyz = bhi + ws.nbmax;                                                  // [nbmax] candidate x,y,z,key bits
+    float4* cxyz = bhi + ws.nbmax;                                                  // [nbmax] candidate x,y,z,sorted position bits
     int* alist = reinterpret_cast<int*>(cxyz + ws.nbmax);                           // [nbmax] active buckets
 
     const float4* __restrict__ pa = ws.pa + static_cast<size_t>(cloud) * (ws.stride / 2);
-    const float4* __restrict__ pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
-    float2* tv2 = ws.tv + static_cast<size_t>(cloud) * (ws.stride / 2);
+    float4* pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
+    const int2* __restrict__ keys = ws.keys + static_cast<size_t>(cloud) * (ws.stride / 2);
+    const int* __restrict__ key = reinterpret_cast<const int*>(keys);
 
     // ---- owner ranges: warp w owns buckets [r0, r1); lane l looks after r0 + l, r0 + l + 32, ... -------------
     const int per = (nb + kMNW - 1) / kMNW;
@@ -416,14 +469,14 @@ fps_bucket_kernel(const float* __restrict__ xyz, const int* __restrict__ offset,
     uhx = warp_max(uhx); uhy = warp_max(uhy); uhz = warp_max(uhz);
 
     auto refresh_range = [&]() {          // best candidate over the owned buckets -> wres[warp]
-        int bv = INT_MIN, bkey = INT_MAX, bbk = r0;
+        int bv = INT_MIN, bpos = -1, bbk = r0;
         for (int bk = r0 + lane; bk < r1; bk += 32) {
-            const int v = __float_as_int(bhi[bk].w), k = __float_as_int(cxyz[bk].w);
-            if (v > bv || (v == bv && k < bkey)) { bv = v; bkey = k; bbk = bk; }
+            const int v = __float_as_int(bhi[bk].w), p = __float_as_int(cxyz[bk].w);
+            if (v > bv || (v == bv && key_at(key, p) < key_at(key, bpos))) { bv = v; bpos = p; bbk = bk; }
         }
-        const int wv = __reduce_max_sync(FULL, bv);
-        const int wk = __reduce_min_sync(FULL, bv == wv ? bkey : INT_MAX);
-        if (bv == wv && bkey == wk) wres[warp] = make_int4(wv, wk, bbk, 0);
+        int wv;
+        const int wl = warp_best_lane(bv, bpos, key, wv);
+        if (lane == wl) wres[warp] = make_int4(wv, bpos, bbk, 0);
         return wv;
     };
     float range_thr = skip_threshold(__int_as_float(refresh_range()));     // r0 == r1: INT_MIN -> negative -> -1
@@ -461,15 +514,13 @@ fps_bucket_kernel(const float* __restrict__ xyz, const int* __restrict__ offset,
         for (int a0 = warp; a0 < na; a0 += kMNW * kBatch) {
             int bk[kBatch];
             float4 A[kBatch], B[kBatch];
-            float2 T[kBatch];
 #pragma unroll
             for (int u = 0; u < kBatch; ++u) {
                 const int a = a0 + u * kMNW;
                 bk[u] = a < na ? alist[a] : -1;
                 if (bk[u] >= 0) {
                     A[u] = __ldg(pa + bk[u] * 32 + lane);
-                    B[u] = __ldg(pb + bk[u] * 32 + lane);
-                    T[u] = __ldcg(tv2 + bk[u] * 32 + lane);
+                    B[u] = __ldcg(pb + bk[u] * 32 + lane);
                 }
             }
 #pragma unroll
@@ -482,17 +533,14 @@ fps_bucket_kernel(const float* __restrict__ xyz, const int* __restrict__ offset,
                 d = fma2(dz, dz, d);
                 float d0, d1;
                 unpack2(d, d0, d1);
-                const float n0 = fminf(d0, T[u].x), n1 = fminf(d1, T[u].y);
-                if (n0 < T[u].x || n1 < T[u].y) __stcg(tv2 + bk[u] * 32 + lane, make_float2(n0, n1));
-                const int b0 = __float_as_int(n0), b1 = __float_as_int(n1);          // pads stay at -1
-                const int k0 = __float_as_int(B[u].z), k1 = __float_as_int(B[u].w);
-                const bool take1 = b1 > b0 || (b1 == b0 && k1 < k0);
-                const int bl = take1 ? b1 : b0, kl = take1 ? k1 : k0;
-                const int wmax = __reduce_max_sync(FULL, bl);
-                const int wkey = __reduce_min_sync(FULL, bl == wmax ? kl : INT_MAX);
-                if (bl == wmax && kl == wkey) {
+                const float n0 = fminf(d0, B[u].z), n1 = fminf(d1, B[u].w);
+                if (n0 < B[u].z || n1 < B[u].w) __stcg(reinterpret_cast<float2*>(pb + bk[u] * 32 + lane) + 1, make_float2(n0, n1));
+                int wmax;
+                bool take1;
+                const int wl = bucket_best(n0, n1, keys + bk[u] * 32 + lane, wmax, take1);
+                if (lane == wl) {
                     cxyz[bk[u]] = make_float4(take1 ? A[u].y : A[u].x, take1 ? A[u].w : A[u].z, take1 ? B[u].y : B[u].x,
-                                              __int_as_float(wkey));
+                                              __int_as_float(bk[u] * kBP + 2 * lane + (take1 ? 1 : 0)));
                     bhi[bk[u]].w = __int_as_float(wmax);
                     blo[bk[u]].w = skip_threshold(__int_as_float(wmax));
                 }
@@ -505,28 +553,19 @@ fps_bucket_kernel(const float* __restrict__ xyz, const int* __restrict__ offset,
         if (dirty) range_thr = skip_threshold(__int_as_float(refresh_range()));
         __syncthreads();
         {
-            int4 c = make_int4(INT_MIN, INT_MAX, 0, 0);
+            int4 c = make_int4(INT_MIN, -1, 0, 0);
             if (lane < kMNW) c = wres[lane];
-            const int gv = __reduce_max_sync(FULL, c.x);
-            const int gk = __reduce_min_sync(FULL, c.x == gv ? c.y : INT_MAX);
-            const int src = __ffs(__ballot_sync(FULL, c.x == gv && c.y == gk)) - 1;
+            int gv;
+            const int src = warp_best_lane(c.x, c.y, key, gv);
             const int bstar = __shfl_sync(FULL, c.z, src);
             const float4 w = cxyz[bstar];
             ox = w.x; oy = w.y; oz = w.z;
-            if (tid == 0) idx[start_m + it] = start_n + key_to_index(__float_as_int(w.w), bs_log2);
+            if (tid == 0) idx[start_m + it] = __float_as_int(w.w);
         }
     }
 
-    if (tmp) {
-        __syncthreads();
-        for (int q = tid; q < nb * 32; q += kMT) {           // q = bucket * 32 + lane
-            const float4 B = __ldg(pb + q);
-            const float2 T = __ldcg(tv2 + q);
-            const int k0 = __float_as_int(B.z), k1 = __float_as_int(B.w);
-            if (k0 != INT_MAX) tmp[start_n + key_to_index(k0, bs_log2)] = T.x;
-            if (k1 != INT_MAX) tmp[start_n + key_to_index(k1, bs_log2)] = T.y;
-        }
-    }
+    positions_to_indices(idx + start_m, m, start_n, key, bs_log2, tid, kMT);
+    if (tmp) write_tmp(tmp, start_n, nb, pb, keys, bs_log2, tid, kMT);
 }
 
 // ---- single-barrier main kernel ("v2") ------------------------------------------------------------------------------------
@@ -545,7 +584,7 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
 {
     constexpr int kMT = MT_, kMNW = MT_ / 32;
     extern __shared__ __align__(16) unsigned char dyn[];
-    struct Slot { int v, k; float x, y, z; int pad[3]; };
+    struct Slot { int v, p; float x, y, z; int pad[3]; };     // value bits, sorted position, coordinates
     __shared__ Slot slot[2][kMNW];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -561,11 +600,12 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
     const int nb = (n + kBP - 1) / kBP;
     float4* blo = reinterpret_cast<float4*>(dyn);                                   // [nbmax] box min, w = skip threshold
     float4* bhi = blo + ws.nbmax;                                                   // [nbmax] box max, w = candidate value bits
-    float4* cxyz = bhi + ws.nbmax;                                                  // [nbmax] candidate x,y,z,key bits
+    float4* cxyz = bhi + ws.nbmax;                                                  // [nbmax] candidate x,y,z,sorted position bits
 
     const float4* __restrict__ pa = ws.pa + static_cast<size_t>(cloud) * (ws.stride / 2);
-    const float4* __restrict__ pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
-    float2* tv2 = ws.tv + static_cast<size_t>(cloud) * (ws.stride / 2);
+    float4* pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
+    const int2* __restrict__ keys = ws.keys + static_cast<size_t>(cloud) * (ws.stride / 2);
+    const int* __restrict__ key = reinterpret_cast<const int*>(keys);
     {
         const float4* glo = ws.box_lo + static_cast<size_t>(cloud) * ws.nbmax;
         const float4* ghi = ws.box_hi + static_cast<size_t>(cloud) * ws.nbmax;
@@ -579,22 +619,19 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
     __syncthreads();
 
     // best candidate over this warp's buckets (warp, warp + W, ...) -> registers of every lane
-    int my_v = INT_MIN, my_k = INT_MAX;
+    int my_v = INT_MIN, my_p = -1;
     float my_x = 0.f, my_y = 0.f, my_z = 0.f;
     auto refresh_own = [&]() {
-        int bv = INT_MIN, bkey = INT_MAX, bbk = -1;
+        int bv = INT_MIN, bpos = -1, bbk = -1;
         for (int bk = warp + kMNW * lane; bk < nb; bk += kMNW * 32) {
-            const int v = __float_as_int(bhi[bk].w), k = __float_as_int(cxyz[bk].w);
-            if (v > bv || (v == bv && k < bkey)) { bv = v; bkey = k; bbk = bk; }
+            const int v = __float_as_int(bhi[bk].w), p = __float_as_int(cxyz[bk].w);
+            if (v > bv || (v == bv && key_at(key, p) < key_at(key, bpos))) { bv = v; bpos = p; bbk = bk; }
         }
-        my_v = __reduce_max_sync(FULL, bv);
-        my_k = __reduce_min_sync(FULL, bv == my_v ? bkey : INT_MAX);
-        const int src = __ffs(__ballot_sync(FULL, bv == my_v && bkey == my_k && bbk >= 0)) - 1;
+        const int src = warp_best_lane(bv, bpos, key, my_v);
+        my_p = __shfl_sync(FULL, bpos, src);
+        const int wb = __shfl_sync(FULL, bbk, src);
         float4 w = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (src >= 0) {
-            const int wb = __shfl_sync(FULL, bbk, src);
-            w = cxyz[wb];
-        }
+        if (wb >= 0) w = cxyz[wb];
         my_x = w.x; my_y = w.y; my_z = w.z;
     };
     refresh_own();
@@ -618,7 +655,6 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
             while (mask) {
                 int bk[kBatch];
                 float4 A[kBatch], B[kBatch];
-                float2 T[kBatch];
 #pragma unroll
                 for (int u = 0; u < kBatch; ++u) {
                     if (mask) {
@@ -626,8 +662,7 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
                         mask &= mask - 1;
                         bk[u] = base + kMNW * l;
                         A[u] = __ldg(pa + bk[u] * 32 + lane);
-                        B[u] = __ldg(pb + bk[u] * 32 + lane);
-                        T[u] = __ldcg(tv2 + bk[u] * 32 + lane);
+                        B[u] = __ldcg(pb + bk[u] * 32 + lane);
                     } else {
                         bk[u] = -1;
                     }
@@ -642,17 +677,14 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
                     d = fma2(dz, dz, d);
                     float d0, d1;
                     unpack2(d, d0, d1);
-                    const float n0 = fminf(d0, T[u].x), n1 = fminf(d1, T[u].y);
-                    if (n0 < T[u].x || n1 < T[u].y) __stcg(tv2 + bk[u] * 32 + lane, make_float2(n0, n1));
-                    const int b0 = __float_as_int(n0), b1 = __float_as_int(n1);          // pads stay at -1
-                    const int k0 = __float_as_int(B[u].z), k1 = __float_as_int(B[u].w);
-                    const bool take1 = b1 > b0 || (b1 == b0 && k1 < k0);
-                    const int bl = take1 ? b1 : b0, kl = take1 ? k1 : k0;
-                    const int wmax = __reduce_max_sync(FULL, bl);
-                    const int wkey = __reduce_min_sync(FULL, bl == wmax ? kl : INT_MAX);
-                    if (bl == wmax && kl == wkey) {
+                    const float n0 = fminf(d0, B[u].z), n1 = fminf(d1, B[u].w);
+                    if (n0 < B[u].z || n1 < B[u].w) __stcg(reinterpret_cast<float2*>(pb + bk[u] * 32 + lane) + 1, make_float2(n0, n1));
+                    int wmax;
+                    bool take1;
+                    const int wl = bucket_best(n0, n1, keys + bk[u] * 32 + lane, wmax, take1);
+                    if (lane == wl) {
                         cxyz[bk[u]] = make_float4(take1 ? A[u].y : A[u].x, take1 ? A[u].w : A[u].z, take1 ? B[u].y : B[u].x,
-                                                  __int_as_float(wkey));
+                                                  __int_as_float(bk[u] * kBP + 2 * lane + (take1 ? 1 : 0)));
                         bhi[bk[u]].w = __int_as_float(wmax);
                         blo[bk[u]].w = skip_threshold(__int_as_float(wmax));
                     }
@@ -665,29 +697,20 @@ fps_bucket_kernel2(const float* __restrict__ xyz, const int* __restrict__ offset
             refresh_own();
         }
         Slot* sl = slot[it & 1];
-        if (lane == 0) { sl[warp].v = my_v; sl[warp].k = my_k; sl[warp].x = my_x; sl[warp].y = my_y; sl[warp].z = my_z; }
+        if (lane == 0) { sl[warp].v = my_v; sl[warp].p = my_p; sl[warp].x = my_x; sl[warp].y = my_y; sl[warp].z = my_z; }
         __syncthreads();
         {
-            int cv = INT_MIN, ck = INT_MAX;
-            if (lane < kMNW) { cv = sl[lane].v; ck = sl[lane].k; }
-            const int gv = __reduce_max_sync(FULL, cv);
-            const int gk = __reduce_min_sync(FULL, cv == gv ? ck : INT_MAX);
-            const int src = __ffs(__ballot_sync(FULL, cv == gv && ck == gk)) - 1;
+            int cv = INT_MIN, cp = -1;
+            if (lane < kMNW) { cv = sl[lane].v; cp = sl[lane].p; }
+            int gv;
+            const int src = warp_best_lane(cv, cp, key, gv);
             ox = sl[src].x; oy = sl[src].y; oz = sl[src].z;
-            if (tid == 0) idx[start_m + it] = start_n + key_to_index(gk, bs_log2);
+            if (tid == 0) idx[start_m + it] = sl[src].p;
         }
     }
 
-    if (tmp) {
-        __syncthreads();
-        for (int q = tid; q < nb * 32; q += kMT) {           // q = bucket * 32 + lane
-            const float4 B = __ldg(pb + q);
-            const float2 T = __ldcg(tv2 + q);
-            const int k0 = __float_as_int(B.z), k1 = __float_as_int(B.w);
-            if (k0 != INT_MAX) tmp[start_n + key_to_index(k0, bs_log2)] = T.x;
-            if (k1 != INT_MAX) tmp[start_n + key_to_index(k1, bs_log2)] = T.y;
-        }
-    }
+    positions_to_indices(idx + start_m, m, start_n, key, bs_log2, tid, kMT);
+    if (tmp) write_tmp(tmp, start_n, nb, pb, keys, bs_log2, tid, kMT);
 }
 
 // ---- register-resident bucket tables ("v3") --------------------------------------------------------------------------------
@@ -703,7 +726,7 @@ fps_bucket_kernel3(const float* __restrict__ xyz, const int* __restrict__ offset
                    float* tmp, int* __restrict__ idx, BucketWs ws, int bs_log2)
 {
     constexpr int kMT = MT_, kMNW = MT_ / 32;
-    struct Slot { int v, k; float x, y, z; int pad[3]; };
+    struct Slot { int v, p; float x, y, z; int pad[3]; };     // value bits, sorted position, coordinates
     __shared__ Slot slot[2][kMNW];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -718,10 +741,11 @@ fps_bucket_kernel3(const float* __restrict__ xyz, const int* __restrict__ offset
 
     const int nb = (n + kBP - 1) / kBP;
     const float4* __restrict__ pa = ws.pa + static_cast<size_t>(cloud) * (ws.stride / 2);
-    const float4* __restrict__ pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
-    float2* tv2 = ws.tv + static_cast<size_t>(cloud) * (ws.stride / 2);
+    float4* pb = ws.pb + static_cast<size_t>(cloud) * (ws.stride / 2);
+    const int2* __restrict__ keys = ws.keys + static_cast<size_t>(cloud) * (ws.stride / 2);
+    const int* __restrict__ key = reinterpret_cast<const int*>(keys);
 
-    // own buckets: bucket (warp + W * (lane + 32 j)), j < BPL
+    // own buckets: bucket (warp + W * (lane + 32 j)), j < BPL; ck = sorted position of the candidate
     float lx[BPL], ly[BPL], lz[BPL], hx[BPL], hy[BPL], hz[BPL], thr[BPL], cx[BPL], cy[BPL], cz[BPL];
     int cv[BPL], ck[BPL];
     {
@@ -738,7 +762,7 @@ fps_bucket_kernel3(const float* __restrict__ xyz, const int* __restrict__ offset
                 cx[j] = c.x; cy[j] = c.y; cz[j] = c.z; ck[j] = __float_as_int(c.w);
             } else {
                 lx[j] = ly[j] = lz[j] = INFINITY; hx[j] = hy[j] = hz[j] = -INFINITY; thr[j] = -1.f;     // never active
-                cv[j] = INT_MIN; ck[j] = INT_MAX; cx[j] = cy[j] = cz[j] = 0.f;
+                cv[j] = INT_MIN; ck[j] = -1; cx[j] = cy[j] = cz[j] = 0.f;
             }
         }
     }
@@ -754,7 +778,6 @@ fps_bucket_kernel3(const float* __restrict__ xyz, const int* __restrict__ offset
             while (mask) {
                 int ol[kBatch];                               // owner lanes of the buckets in flight
                 float4 A[kBatch], B[kBatch];
-                float2 T[kBatch];
 #pragma unroll
                 for (int u = 0; u < kBatch; ++u) {
                     if (mask) {
@@ -762,8 +785,7 @@ fps_bucket_kernel3(const float* __restrict__ xyz, const int* __restrict__ offset
                         mask &= mask - 1;
                         const int bk = warp + kMNW * (ol[u] + 32 * j);
                         A[u] = __ldg(pa + bk * 32 + lane);
-                        B[u] = __ldg(pb + bk * 32 + lane);
-                        T[u] = __ldcg(tv2 + bk * 32 + lane);
+                        B[u] = __ldcg(pb + bk * 32 + lane);
                     } else {
                         ol[u] = -1;
                     }
@@ -779,53 +801,41 @@ fps_bucket_kernel3(const float* __restrict__ xyz, const int* __restrict__ offset
                     d = fma2(dz, dz, d);
                     float d0, d1;
                     unpack2(d, d0, d1);
-                    const float n0 = fminf(d0, T[u].x), n1 = fminf(d1, T[u].y);
-                    if (n0 < T[u].x || n1 < T[u].y) __stcg(tv2 + bk * 32 + lane, make_float2(n0, n1));
-                    const int b0 = __float_as_int(n0), b1 = __float_as_int(n1);          // pads stay at -1
-                    const int k0 = __float_as_int(B[u].z), k1 = __float_as_int(B[u].w);
-                    const bool take1 = b1 > b0 || (b1 == b0 && k1 < k0);
-                    const int bl = take1 ? b1 : b0, kl = take1 ? k1 : k0;
-                    const int wmax = __reduce_max_sync(FULL, bl);
-                    const int wkey = __reduce_min_sync(FULL, bl == wmax ? kl : INT_MAX);
-                    const int wl = __ffs(__ballot_sync(FULL, bl == wmax && kl == wkey)) - 1;      // the lane holding the candidate point
+                    const float n0 = fminf(d0, B[u].z), n1 = fminf(d1, B[u].w);
+                    if (n0 < B[u].z || n1 < B[u].w) __stcg(reinterpret_cast<float2*>(pb + bk * 32 + lane) + 1, make_float2(n0, n1));
+                    int wmax;
+                    bool take1;
+                    const int wl = bucket_best(n0, n1, keys + bk * 32 + lane, wmax, take1);      // the lane holding the candidate point
                     const float nx = __shfl_sync(FULL, take1 ? A[u].y : A[u].x, wl), ny = __shfl_sync(FULL, take1 ? A[u].w : A[u].z, wl),
                                 nz = __shfl_sync(FULL, take1 ? B[u].y : B[u].x, wl);
-                    if (lane == ol[u]) { cv[j] = wmax; ck[j] = wkey; thr[j] = skip_threshold(__int_as_float(wmax)); cx[j] = nx; cy[j] = ny; cz[j] = nz; }
+                    const int np = __shfl_sync(FULL, bk * kBP + 2 * lane + (take1 ? 1 : 0), wl);
+                    if (lane == ol[u]) { cv[j] = wmax; ck[j] = np; thr[j] = skip_threshold(__int_as_float(wmax)); cx[j] = nx; cy[j] = ny; cz[j] = nz; }
                 }
             }
         }
         // ---- this warp's candidate: registers only -------------------------------------------------------------------------
-        int bv = cv[0], bkey = ck[0];
+        int bv = cv[0], bpos = ck[0];
         float bx = cx[0], by = cy[0], bz = cz[0];
 #pragma unroll
         for (int j = 1; j < BPL; ++j)
-            if (cv[j] > bv || (cv[j] == bv && ck[j] < bkey)) { bv = cv[j]; bkey = ck[j]; bx = cx[j]; by = cy[j]; bz = cz[j]; }
-        const int wv = __reduce_max_sync(FULL, bv);
-        const int wk = __reduce_min_sync(FULL, bv == wv ? bkey : INT_MAX);
+            if (cv[j] > bv || (cv[j] == bv && key_at(key, ck[j]) < key_at(key, bpos))) { bv = cv[j]; bpos = ck[j]; bx = cx[j]; by = cy[j]; bz = cz[j]; }
+        int wv;
+        const int wl = warp_best_lane(bv, bpos, key, wv);
         Slot* sl = slot[it & 1];
-        if (bv == wv && bkey == wk) { sl[warp].v = wv; sl[warp].k = wk; sl[warp].x = bx; sl[warp].y = by; sl[warp].z = bz; }
+        if (lane == wl) { sl[warp].v = wv; sl[warp].p = bpos; sl[warp].x = bx; sl[warp].y = by; sl[warp].z = bz; }
         __syncthreads();
         {
-            int sv = INT_MIN, sk = INT_MAX;
-            if (lane < kMNW) { sv = sl[lane].v; sk = sl[lane].k; }
-            const int gv = __reduce_max_sync(FULL, sv);
-            const int gk = __reduce_min_sync(FULL, sv == gv ? sk : INT_MAX);
-            const int src = __ffs(__ballot_sync(FULL, sv == gv && sk == gk)) - 1;
+            int sv = INT_MIN, sp = -1;
+            if (lane < kMNW) { sv = sl[lane].v; sp = sl[lane].p; }
+            int gv;
+            const int src = warp_best_lane(sv, sp, key, gv);
             ox = sl[src].x; oy = sl[src].y; oz = sl[src].z;
-            if (tid == 0) idx[start_m + it] = start_n + key_to_index(gk, bs_log2);
+            if (tid == 0) idx[start_m + it] = sl[src].p;
         }
     }
 
-    if (tmp) {
-        __syncthreads();
-        for (int q = tid; q < nb * 32; q += kMT) {           // q = bucket * 32 + lane
-            const float4 B = __ldg(pb + q);
-            const float2 T = __ldcg(tv2 + q);
-            const int k0 = __float_as_int(B.z), k1 = __float_as_int(B.w);
-            if (k0 != INT_MAX) tmp[start_n + key_to_index(k0, bs_log2)] = T.x;
-            if (k1 != INT_MAX) tmp[start_n + key_to_index(k1, bs_log2)] = T.y;
-        }
-    }
+    positions_to_indices(idx + start_m, m, start_n, key, bs_log2, tid, kMT);
+    if (tmp) write_tmp(tmp, start_n, nb, pb, keys, bs_log2, tid, kMT);
 }
 
 template <int MT_, int BPL>
@@ -873,7 +883,7 @@ int fps_bucket_launch(int b, int n_max, const float* xyz, const int* offset, con
     // one stream-ordered allocation, carved
     size_t off = 0;
     auto take = [&off](size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~static_cast<size_t>(255); return o; };
-    const size_t o_pa = take(pts / 2 * sizeof(float4)), o_pb = take(pts / 2 * sizeof(float4)), o_t = take(pts / 2 * sizeof(float2)),
+    const size_t o_pa = take(pts / 2 * sizeof(float4)), o_pb = take(pts / 2 * sizeof(float4)), o_k = take(pts / 2 * sizeof(int2)),
                  o_ka = take(smem_sort ? 0 : pts * sizeof(uint2)), o_kb = take(smem_sort ? 0 : pts * sizeof(uint2)),
                  o_lo = take(nbt * sizeof(float4)), o_hi = take(nbt * sizeof(float4)), o_bx = take(nbt * sizeof(float4));
     keep_async_pool();
@@ -882,7 +892,7 @@ int fps_bucket_launch(int b, int n_max, const float* xyz, const int* offset, con
     if (e != cudaSuccess) { set_error("furthestsampling: workspace of %zu bytes: %s", off, cudaGetErrorString(e)); (void)cudaGetLastError(); return TGN_ERR_CUDA; }
     ws.pa = reinterpret_cast<float4*>(base + o_pa);
     ws.pb = reinterpret_cast<float4*>(base + o_pb);
-    ws.tv = reinterpret_cast<float2*>(base + o_t);
+    ws.keys = reinterpret_cast<int2*>(base + o_k);
     ws.key_a = reinterpret_cast<uint2*>(base + o_ka);
     ws.key_b = reinterpret_cast<uint2*>(base + o_kb);
     ws.box_lo = reinterpret_cast<float4*>(base + o_lo);
