@@ -115,6 +115,16 @@ size_t tgn_knn_f64_bytes(int n);
 int tgn_knn_f64(int n, int m, int k, const double *xyz, const double *queries, void *workspace, const int *labels, long long *idx,
                 double *dist, int *nn0, int *agree, void *stream);
 
+/* The same kNN with the grid built once and queried many times (KDTree(X) once, .query(...) per query set): tgn_knn_f64_build
+ * writes the grid of xyz (n,3) float64 DEVICE into a caller-owned DEVICE workspace of tgn_knn_f64_bytes(n) bytes;
+ * tgn_knn_f64_query answers queries (m,3) against it without writing to it (xyz and n are those of the build; any number of
+ * queries may share one built workspace).  tgn_knn_f64 is build + query.  Outputs as above, plus tie (m) bytes, optional:
+ * tie[i] = 1 exactly when two adjacent keys among query i's min(k+1, n) smallest (d2, index) have equal d2, else 0.  A row with
+ * tie[i] = 0 has one answer under every tie-break rule (sklearn's KDTree returns exactly it).  With tie, 1 <= k <= 63. */
+int tgn_knn_f64_build(int n, const double *xyz, void *workspace, void *stream);
+int tgn_knn_f64_query(int n, int m, int k, const double *xyz, const double *queries, const void *workspace, const int *labels,
+                      long long *idx, double *dist, int *nn0, int *agree, unsigned char *tie, void *stream);
+
 /* kNN through a per-segment uniform grid: identical answers to tgn_knnquery (distinct distances: order-independent;
  * ties among the k+1 best: the query is re-run with the reference's index-order heap), ~100x fewer distance evaluations
  * on 24k-point clouds.  The grid depends only on (xyz, offset): build it once into a caller-owned DEVICE workspace of

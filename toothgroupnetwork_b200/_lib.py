@@ -25,6 +25,8 @@ _SIGS = {
     "tgn_pt_layer_set_cta_threshold": [_i],
     "tgn_dbscan": [_i, _vp, ctypes.c_double, _i, _vp, _vp, _vp, _vp, _vp],
     "tgn_knn_f64": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "tgn_knn_f64_build": [_i, _vp, _vp, _vp],
+    "tgn_knn_f64_query": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_csr_build": [ctypes.c_longlong, _i, _vp, _vp, _vp],
     "tgn_gather_backward_det": [ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp],
     "tgn_weighted_gather_backward_det": [ctypes.c_longlong, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],

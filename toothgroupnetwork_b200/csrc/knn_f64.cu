@@ -19,6 +19,11 @@
 //     L is shrunk by a slack far larger than the rounding of the cell assignment and of L itself, and the search stops when
 //     d2[k-th best] < L^2 * (1 - 1e-12) -- strictly below every d2 an unvisited point can produce -- or when the cube covers
 //     the grid.  Stopping later only costs time.
+//   * build once, query many times: tgn_knn_f64_build writes the grid into a caller-owned workspace and tgn_knn_f64_query only
+//     reads it, so one point set serves any number of query sets and k;
+//   * tie flag (optional): the warp keeps the min(k+1, n) best keys and flags the query when two adjacent ones have equal d2.
+//     An unflagged query's k neighbours, and their order, are the same under every tie-break rule, so scikit-learn's KDTree
+//     (which keeps whichever tied point its walk meets first) returns exactly them; flagged rows are for the caller to resolve.
 #include <climits>
 #include <cmath>
 
@@ -212,10 +217,11 @@ __device__ __forceinline__ double sq_dist(double qx, double qy, double qz, const
 
 __device__ __forceinline__ bool key_less(double d, int i, double od, int oi) { return d < od || (d == od && i < oi); }
 
-template <int EPL>
-__global__ void __launch_bounds__(kWarps * 32, 4)      // four CTAs per SM: ptxas then keeps everything in registers
-knn_f64_query_kernel(int n, int m, int k, const double* __restrict__ queries, const F64Ws ws, const int* __restrict__ labels,
-                     long long* __restrict__ idx, double* __restrict__ dist, int* __restrict__ nn0, int* __restrict__ agree)
+// One warp per query.  TIE: the list holds keep = min(k+1, n) entries instead of k and tie[q] reports an equal adjacent pair of d2.
+template <int EPL, bool TIE>
+__device__ __forceinline__ void knn_f64_query(int n, int m, int k, const double* __restrict__ queries, const F64Ws& ws,
+                                              const int* __restrict__ labels, long long* __restrict__ idx, double* __restrict__ dist,
+                                              int* __restrict__ nn0, int* __restrict__ agree, unsigned char* __restrict__ tie)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int q = blockIdx.x * kWarps + warp;
@@ -229,8 +235,9 @@ knn_f64_query_kernel(int n, int m, int k, const double* __restrict__ queries, co
     int li[EPL];
 #pragma unroll
     for (int e = 0; e < EPL; ++e) { ld[e] = INFINITY; li[e] = INT_MAX; }
-    const int kth_lane = (k - 1) / EPL, kth_sub = (k - 1) % EPL;
-    double tau_d = INFINITY;                              // key of the k-th entry
+    const int keep = TIE ? min(k + 1, n) : k;
+    const int kth_lane = (keep - 1) / EPL, kth_sub = (keep - 1) % EPL;
+    double tau_d = INFINITY;                              // key of the keep-th entry
     int tau_i = INT_MAX;
 
     auto scan_range = [&](int p0, int p1) {               // candidates sorted[p0, p1)
@@ -334,6 +341,34 @@ knn_f64_query_kernel(int n, int m, int k, const double* __restrict__ queries, co
         if (lane == 0 && agree) agree[q] = count;
     }
     if (lane == 0 && nn0) nn0[q] = first;
+    if constexpr (TIE) {
+        const double prev = __shfl_up_sync(FULL, ld[EPL - 1], 1);           // the entry before this lane's first
+        bool eq = false;
+#pragma unroll
+        for (int e = 0; e < EPL; ++e) {
+            const int ent = lane * EPL + e;
+            if (ent >= 1 && ent < keep) eq |= (e ? ld[e - 1] : prev) == ld[e];  // d2 >= +0 and finite: == is bitwise equality
+        }
+        const bool any = __any_sync(FULL, eq);
+        if (lane == 0) tie[q] = any ? 1 : 0;
+    }
+}
+
+template <int EPL>
+__global__ void __launch_bounds__(kWarps * 32, 4)      // four CTAs per SM: ptxas then keeps everything in registers
+knn_f64_query_kernel(int n, int m, int k, const double* __restrict__ queries, const F64Ws ws, const int* __restrict__ labels,
+                     long long* __restrict__ idx, double* __restrict__ dist, int* __restrict__ nn0, int* __restrict__ agree)
+{
+    knn_f64_query<EPL, false>(n, m, k, queries, ws, labels, idx, dist, nn0, agree, nullptr);
+}
+
+template <int EPL>
+__global__ void __launch_bounds__(kWarps * 32, 4)
+knn_f64_tie_query_kernel(int n, int m, int k, const double* __restrict__ queries, const F64Ws ws, const int* __restrict__ labels,
+                         long long* __restrict__ idx, double* __restrict__ dist, int* __restrict__ nn0, int* __restrict__ agree,
+                         unsigned char* __restrict__ tie)
+{
+    knn_f64_query<EPL, true>(n, m, k, queries, ws, labels, idx, dist, nn0, agree, tie);
 }
 
 }  // namespace
@@ -344,6 +379,56 @@ extern "C" {
 size_t tgn_knn_f64_bytes(int n)
 {
     return tgn::carve(n > 0 ? n : 1, nullptr, nullptr);
+}
+
+int tgn_knn_f64_build(int n, const double* xyz, void* workspace, void* stream)
+{
+    using namespace tgn;
+    if (n < 1) { set_error("knn_f64_build: need n >= 1 (n=%d)", n); return TGN_ERR_INVALID; }
+    if (!xyz || !workspace) { set_error("knn_f64_build: null argument"); return TGN_ERR_INVALID; }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    F64Ws ws{};
+    carve(n, &ws, static_cast<unsigned char*>(workspace));
+    knn_f64_setup_kernel<<<1, kScanThreads, 0, st>>>(n, xyz, ws);
+    int rc = check_launch("knn_f64_setup_kernel");
+    if (rc != TGN_OK) return rc;
+    const int blocks = (n + 255) / 256;
+    knn_f64_count_kernel<<<blocks, 256, 0, st>>>(n, xyz, ws);
+    if ((rc = check_launch("knn_f64_count_kernel")) != TGN_OK) return rc;
+    knn_f64_scan_kernel<<<1, kScanThreads, 0, st>>>(n, ws);
+    if ((rc = check_launch("knn_f64_scan_kernel")) != TGN_OK) return rc;
+    knn_f64_scatter_kernel<<<blocks, 256, 0, st>>>(n, xyz, ws);
+    return check_launch("knn_f64_scatter_kernel");
+}
+
+int tgn_knn_f64_query(int n, int m, int k, const double* xyz, const double* queries, const void* workspace, const int* labels,
+                      long long* idx, double* dist, int* nn0, int* agree, unsigned char* tie, void* stream)
+{
+    using namespace tgn;
+    const int max_k = tie ? kMaxK - 1 : kMaxK;            // the tie flag needs one more list entry
+    if (n < 1 || m < 0 || k < 1 || k > max_k || k > n) {
+        set_error("knn_f64_query: need 1 <= k <= min(n, %d)%s, m >= 0 (n=%d m=%d k=%d)", max_k, tie ? " with tie" : "", n, m, k);
+        return TGN_ERR_INVALID;
+    }
+    if (m == 0) return TGN_OK;
+    if (!xyz || !queries || !workspace) { set_error("knn_f64_query: null argument"); return TGN_ERR_INVALID; }
+    if (agree && !labels) { set_error("knn_f64_query: agree needs labels"); return TGN_ERR_INVALID; }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    F64Ws ws{};
+    carve(n, &ws, static_cast<unsigned char*>(const_cast<void*>(workspace)));   // read only below
+    const int grid = (m + kWarps - 1) / kWarps;
+    if (tie) {
+        if (k + 1 <= 32)
+            knn_f64_tie_query_kernel<1><<<grid, kWarps * 32, 0, st>>>(n, m, k, queries, ws, labels, idx, dist, nn0, agree, tie);
+        else
+            knn_f64_tie_query_kernel<2><<<grid, kWarps * 32, 0, st>>>(n, m, k, queries, ws, labels, idx, dist, nn0, agree, tie);
+        return check_launch("knn_f64_tie_query_kernel");
+    }
+    if (k <= 32)
+        knn_f64_query_kernel<1><<<grid, kWarps * 32, 0, st>>>(n, m, k, queries, ws, labels, idx, dist, nn0, agree);
+    else
+        knn_f64_query_kernel<2><<<grid, kWarps * 32, 0, st>>>(n, m, k, queries, ws, labels, idx, dist, nn0, agree);
+    return check_launch("knn_f64_query_kernel");
 }
 
 int tgn_knn_f64(int n, int m, int k, const double* xyz, const double* queries, void* workspace, const int* labels, long long* idx,
@@ -357,25 +442,9 @@ int tgn_knn_f64(int n, int m, int k, const double* xyz, const double* queries, v
     if (m == 0) return TGN_OK;
     if (!xyz || !queries || !workspace) { set_error("knn_f64: null argument"); return TGN_ERR_INVALID; }
     if (agree && !labels) { set_error("knn_f64: agree needs labels"); return TGN_ERR_INVALID; }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    F64Ws ws{};
-    carve(n, &ws, static_cast<unsigned char*>(workspace));
-    knn_f64_setup_kernel<<<1, kScanThreads, 0, st>>>(n, xyz, ws);
-    int rc = check_launch("knn_f64_setup_kernel");
+    const int rc = tgn_knn_f64_build(n, xyz, workspace, stream);
     if (rc != TGN_OK) return rc;
-    const int blocks = (n + 255) / 256;
-    knn_f64_count_kernel<<<blocks, 256, 0, st>>>(n, xyz, ws);
-    if ((rc = check_launch("knn_f64_count_kernel")) != TGN_OK) return rc;
-    knn_f64_scan_kernel<<<1, kScanThreads, 0, st>>>(n, ws);
-    if ((rc = check_launch("knn_f64_scan_kernel")) != TGN_OK) return rc;
-    knn_f64_scatter_kernel<<<blocks, 256, 0, st>>>(n, xyz, ws);
-    if ((rc = check_launch("knn_f64_scatter_kernel")) != TGN_OK) return rc;
-    const int grid = (m + kWarps - 1) / kWarps;
-    if (k <= 32)
-        knn_f64_query_kernel<1><<<grid, kWarps * 32, 0, st>>>(n, m, k, queries, ws, labels, idx, dist, nn0, agree);
-    else
-        knn_f64_query_kernel<2><<<grid, kWarps * 32, 0, st>>>(n, m, k, queries, ws, labels, idx, dist, nn0, agree);
-    return check_launch("knn_f64_query_kernel");
+    return tgn_knn_f64_query(n, m, k, xyz, queries, workspace, labels, idx, dist, nn0, agree, nullptr, stream);
 }
 
 }  // extern "C"

@@ -88,6 +88,22 @@ def accelerate_inference_pipeline(module=None) -> None:
     boundary.accelerate(module)
 
 
+def accelerate_label_transfer(module=None) -> None:
+    """Optional: answer the float64 ``KDTree.query`` calls of the inference pipelines' label transfers on the GPU through
+    ``toothgroupnetwork_b200.neighbors.KDTree`` (the boundary clusters and the final transfer to the mesh,
+    inference_pipeline_tgn.py:107-114, :137-140; the final transfers of inference_pipeline_tsegnet.py:72-74 and
+    inference_pipeline_sem.py:37-39), with the same indices and distances.  Swaps the ``KDTree`` name of
+    ``inference_pipelines.inference_pipeline_tgn`` (imported from ``sys.path`` when no module is passed), and of the tsegnet and
+    sem pipelines when they are already imported.  ``ops_utils`` keeps its own: ``accelerate_ops_utils`` replaces its queries."""
+    from . import neighbors
+    if module is None:
+        module = importlib.import_module("inference_pipelines.inference_pipeline_tgn")
+    neighbors.accelerate(module)
+    for name in ("inference_pipelines.inference_pipeline_tsegnet", "inference_pipelines.inference_pipeline_sem"):
+        if name in sys.modules:
+            neighbors.accelerate(sys.modules[name])
+
+
 def uninstall() -> None:
     for alias in _TARGETS:
         sys.modules.pop(alias, None)
