@@ -125,6 +125,15 @@ int tgn_knn_f64_build(int n, const double *xyz, void *workspace, void *stream);
 int tgn_knn_f64_query(int n, int m, int k, const double *xyz, const double *queries, const void *workspace, const int *labels,
                       long long *idx, double *dist, int *nn0, int *agree, unsigned char *tie, void *stream);
 
+/* Exact feature-space kNN of DGCNN (models/modules/dgcnn.py:4-10): per cloud, the k largest of
+ * v_ij = fl(fl(-xx_j - fl(-2*dot_ij)) - xx_i), dot_ij = the in-order FFMA chain over c, with the indices and values
+ * pairwise_distance.topk(k, dim=-1) returns, without the N x N matrix.  x (b, c, n) float32 DEVICE, element (bi, ci, ni) at
+ * x[bi*stride_b + ci*stride_c + ni*stride_n]; xx (b, n) float32 DEVICE = torch.sum(x**2, dim=1) as the caller computed it;
+ * 1 <= c <= 64, 1 <= k <= 32, n >= k.  Outputs idx (b, n, k) int64 and val (b, n, k) float32 (optional, NULL), in topk's
+ * sorted order (a NaN value is returned as the canonical NaN). */
+int tgn_knn_feat(int b, int n, int c, int k, const float *x, long long stride_b, long long stride_c, long long stride_n,
+                 const float *xx, long long *idx, float *val, void *stream);
+
 /* kNN through a per-segment uniform grid: identical answers to tgn_knnquery (distinct distances: order-independent;
  * ties among the k+1 best: the query is re-run with the reference's index-order heap), ~100x fewer distance evaluations
  * on 24k-point clouds.  The grid depends only on (xyz, offset): build it once into a caller-owned DEVICE workspace of

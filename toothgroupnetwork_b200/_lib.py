@@ -27,6 +27,7 @@ _SIGS = {
     "tgn_knn_f64": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_knn_f64_build": [_i, _vp, _vp, _vp],
     "tgn_knn_f64_query": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "tgn_knn_feat": [_i, _i, _i, _i, _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, _vp, _vp, _vp],
     "tgn_csr_build": [ctypes.c_longlong, _i, _vp, _vp, _vp],
     "tgn_gather_backward_det": [ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp],
     "tgn_weighted_gather_backward_det": [ctypes.c_longlong, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],

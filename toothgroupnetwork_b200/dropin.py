@@ -104,6 +104,17 @@ def accelerate_label_transfer(module=None) -> None:
             neighbors.accelerate(sys.modules[name])
 
 
+def accelerate_dgcnn(module=None) -> None:
+    """Optional: answer the feature-space kNN of the DGCNN model (``knn`` of models/modules/dgcnn.py:4-10, called three times per
+    forward by ``get_graph_feature``) with the exact kernel of ``toothgroupnetwork_b200.dgcnn``: the same indices without the
+    N x N matrix.  Inputs the kernel does not reproduce stay on the module's own ``knn``.  Imports ``models.modules.dgcnn`` from
+    ``sys.path`` when no module is passed."""
+    from . import dgcnn
+    if module is None:
+        module = importlib.import_module("models.modules.dgcnn")
+    dgcnn.accelerate(module)
+
+
 def uninstall() -> None:
     for alias in _TARGETS:
         sys.modules.pop(alias, None)
