@@ -248,6 +248,12 @@ int tgn_sa_group_mlp_max(int B, int N, int S, int K, int D, const float *xyz, co
  *         x[k] = seg_ptr[i][b*seg_batch_stride[i] + n*seg_row_stride[i] + k'*seg_chan_stride[i]] (strides in floats);
  * mode 1: neighbourhood gather, r = ((b*S + s)*K + j): [feats[b, gidx[r], :] | xyz[b, gidx[r]] - new_xyz[b, s]]
  *         (xyz_first = 0, MSG order :285) or [xyz - centre | feats] (xyz_first = 1, SSG order :169); cin = D + 3.
+ * mode 2: DGCNN edge feature (get_graph_feature, models/modules/dgcnn.py:13-41), r = ((b*N + n)*K + j), m = gidx[r] in [0, N):
+ *         [x[b, :, m] - x[b, :, n] | x[b, :, n]] with x = edge_x read through edge_stride = its (b, c, n) strides in floats;
+ *         cin = 2 * edge_C, rows a multiple of N * K.  A row whose m is out of range is a zero row.
+ * in_act: the activation applied after the input BatchNorm: 0 = ReLU, 1 = LeakyReLU (v > 0 ? v : v * in_act_slope).
+ * cloud_bias (optional, (B, cout)): y[c, r] += cloud_bias[r / rows_per_batch, c] after the bias -- an operand segment that is
+ * constant over each cloud's rows, added once in fp32 instead of through the MMAs (tgn_pw_cloud_bias computes it).
  * Outputs, each optional: y (cout, rows); stats (2*cout doubles, ACCUMULATED: caller zeroes) = per-channel
  * sum / sum of squares of y; ymax / ymin (cout, rows/group) = extrema over groups of `group` consecutive rows
  * (the max over the K neighbours must wait for the BatchNorm scale's sign, so both are kept); with
@@ -275,12 +281,19 @@ typedef struct {
     float *ymax, *ymin;
     int group, extrema_atomic;
     int precision;          /* 0 / 3: three bf16 parts per operand, six MMAs per K step (fp32-grade); 2: two parts, three MMAs (~1e-5) */
+    const float *edge_x;    /* mode 2 */
+    long long edge_stride[3];
+    int edge_C;
+    int in_act;
+    float in_act_slope;
+    const float *cloud_bias;
 } tgn_pw_layer_t;
 
-/* Final BatchNorm (+ ReLU) of a chain into a channel-first tensor:
- *   out[b, out_c_offset + c, n] = relu?(scale_c * v + shift_c),  v = src[c, b*rows_per_batch + n]
+/* Final BatchNorm (+ activation) of a chain into a channel-first tensor:
+ *   out[b, out_c_offset + c, n] = act(scale_c * v + shift_c),  v = src[c, b*rows_per_batch + n]
  * or, when ymin != NULL, v = (scale_c >= 0 ? src : ymin)[c, ...] (src = the max).  `affine` as in_affine above
- * (0 = identity), statistics over stat_rows rows. */
+ * (0 = identity), statistics over stat_rows rows.  act: LeakyReLU (v > 0 ? v : v * act_slope) when act == 1, else ReLU
+ * when relu != 0, else none. */
 typedef struct {
     int rows, rows_per_batch, channels, out_channels, out_c_offset, relu;
     const float *src, *ymin;
@@ -291,6 +304,8 @@ typedef struct {
     const float *gamma, *beta;
     float *running_mean, *running_var;
     float eps, momentum;
+    int act;
+    float act_slope;
 } tgn_pw_apply_t;
 
 /* Fused forward of blocks.PointTransformerLayer (models/modules/cbl_point_transformer/blocks.py:14-44; SURVEY 8(f)-3): vector
@@ -329,6 +344,9 @@ int tgn_pw_pack_weights(int cout, int cin, const float *w, void *packed, void *s
 int tgn_pw_layer_forward(const tgn_pw_layer_t *layer, void *stream);
 int tgn_pw_apply(const tgn_pw_apply_t *p, void *stream);
 int tgn_pw_fill(float *ptr, long long n, float value, void *stream);
+/* out[b*cout + c] = sum_k w[c*w_row_stride + k] * g[b*g_batch_stride + k], k < cin, accumulated in fp64 and rounded once */
+int tgn_pw_cloud_bias(int B, int cout, int cin, const float *w, long long w_row_stride, const float *g, long long g_batch_stride,
+                      float *out, void *stream);
 
 #ifdef __cplusplus
 }

@@ -6,7 +6,10 @@
   kernel's FP32 rate (2*B*N^2*C FLOP over its time) as a share of the 67 TFLOP/s data-sheet figure, and the outputs compared
   bitwise;
 * a whole DGCnnModule forward, no-grad with batch-statistics BatchNorm as the sem pipeline runs it, and one training step
-  (forward, cross-entropy, backward), each with and without the drop-in: times, peak memory, cls_pred / loss / gradients bitwise.
+  (forward, cross-entropy, backward), each with and without the drop-in: times, peak memory, cls_pred / loss / gradients bitwise;
+* under "fused_forward" (DESIGN §3.12), for batch-statistics and eval-mode BatchNorm: the no-grad forward of the reference, with the
+  kNN drop-in only, and fused (``accelerate_forward``), timed in the same windows in turn; the peak-memory growth of each; the
+  share of points whose argmax(cls_pred) differs from the reference's; the rows whose layer-2 / layer-3 neighbour sets differ.
 
 The reference's model file comes from the staged snapshot (oracle.ref_models).  Prints one JSON object with the card's name and
 power limit, and also writes it to the file given by --out.
@@ -64,6 +67,91 @@ def load_reference_dgcnn(name):
 
 def bits_equal(a, b):
     return bool(torch.equal(a.view(torch.int32), b.view(torch.int32)))
+
+
+def timed_in_turn(fns, warmup, windows, reps):
+    """median / min / max ms per call of each fn, the windows of the fns alternating"""
+    for fn in fns.values():
+        for _ in range(warmup):
+            fn()
+    torch.cuda.synchronize()
+    times = {tag: [] for tag in fns}
+    for _ in range(windows):
+        for tag, fn in fns.items():
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(reps):
+                fn()
+            b.record()
+            b.synchronize()
+            times[tag].append(a.elapsed_time(b) / reps)
+    out = {}
+    for tag, t in times.items():
+        t.sort()
+        out[tag] = {"median_ms": t[len(t) // 2], "min_ms": t[0], "max_ms": t[-1]}
+    return out
+
+
+def fused_forward_rows(a, ref_mod, knn_mod, x6):
+    fused_mod = load_reference_dgcnn("ref_dgcnn_bench_c")
+    dropin.accelerate_dgcnn_forward(fused_mod)
+    torch.backends.cudnn.deterministic = False
+    rows = {}
+    for bn_mode in ("batch_statistics", "eval"):          # eval mode is refused by dgcnn.fusable: the "fused" model runs the reference
+        torch.manual_seed(0)
+        base = ref_mod.DGCnnModule(None).cuda().train()
+        if bn_mode == "eval":                         # running statistics = the batch statistics of one pass, as after training
+            for name in ("bn1", "bn2", "bn3", "bn4", "bn5", "bn6", "bn7", "bn8"):
+                getattr(base, name).momentum = 1.0
+            with torch.no_grad():
+                base([x6])
+            for name in ("bn1", "bn2", "bn3", "bn4", "bn5", "bn6", "bn7", "bn8"):
+                getattr(base, name).momentum = 0.1
+        models = {}
+        for tag, mod in (("reference", ref_mod), ("knn_only", knn_mod), ("fused", fused_mod)):
+            m = mod.DGCnnModule(None).cuda()
+            m.load_state_dict(base.state_dict())
+            models[tag] = m.train() if bn_mode == "batch_statistics" else m.eval()
+
+        def forward(tag):
+            with torch.no_grad():
+                torch.manual_seed(1)
+                return models[tag]([x6])["cls_pred"]
+
+        row = {}
+        preds = {}
+        for tag in models:
+            forward(tag)
+            preds[tag], row[f"{tag}_peak_growth_bytes"] = peak_growth(lambda: forward(tag))
+        before = L.launch_count()
+        forward("fused")
+        row["fused_launches"] = L.launch_count() - before
+        row["times"] = timed_in_turn({tag: (lambda t=tag: forward(t)) for tag in models}, 2, a.windows, 3)
+        row["fused_speedup_over_knn_only"] = row["times"]["knn_only"]["median_ms"] / row["times"]["fused"]["median_ms"]
+        row["fused_speedup_over_reference"] = row["times"]["reference"]["median_ms"] / row["times"]["fused"]["median_ms"]
+        row["argmax_differs_fraction"] = float((preds["fused"].argmax(1) != preds["reference"].argmax(1)).float().mean())
+        saved = torch.backends.cudnn.allow_tf32
+        torch.backends.cudnn.allow_tf32 = False
+        try:
+            ref_fp32 = forward("reference")
+        finally:
+            torch.backends.cudnn.allow_tf32 = saved
+        row["argmax_differs_fraction_vs_reference_without_tf32"] = float((preds["fused"].argmax(1) != ref_fp32.argmax(1)).float().mean())
+        row["argmax_differs_fraction_reference_tf32_vs_fp32"] = float((preds["reference"].argmax(1) != ref_fp32.argmax(1)).float().mean())
+        # neighbour sets of layers 2 and 3: the reference's own search on its features against the kernel's on the fused ones
+        ref_idx, new_idx = [], []
+        original = ref_mod.knn
+        ref_mod.knn = lambda v, k: ref_idx.append(original(v, k)) or ref_idx[-1]
+        try:
+            forward("reference")
+        finally:
+            ref_mod.knn = original
+        with torch.no_grad():
+            torch.manual_seed(1)
+            dgcnn.forward(models["fused"], [x6], knn=lambda v, k: new_idx.append(dgcnn.knn_features(v, k)) or new_idx[-1])
+        row["neighbour_rows_differing"] = [int((u.sort(-1)[0] != w.sort(-1)[0]).any(-1).sum()) for u, w in zip(ref_idx, new_idx)]
+        rows[bn_mode] = row
+    return rows
 
 
 def main() -> None:
@@ -139,6 +227,8 @@ def main() -> None:
         bits_equal(u, v) for u, v in zip(g0, g1))
     for key in ("forward_no_grad", "train_step"):
         out["model"][f"{key}_speedup"] = out["model"]["reference"][key]["median_ms"] / out["model"]["dropin"][key]["median_ms"]
+
+    out["fused_forward"] = fused_forward_rows(a, ref_mod, new_mod, x6)
 
     if a.out:
         with open(a.out, "w") as f:

@@ -56,6 +56,7 @@ _SIGS = {
     "tgn_pw_layer_forward": [_vp, _vp],
     "tgn_pw_apply": [_vp, _vp],
     "tgn_pw_fill": [_vp, ctypes.c_longlong, _f, _vp],
+    "tgn_pw_cloud_bias": [_i, _i, _i, _vp, ctypes.c_longlong, _vp, ctypes.c_longlong, _vp, _vp],
 }
 
 
@@ -73,6 +74,8 @@ class PwLayer(ctypes.Structure):
         ("in_eps", _f), ("in_momentum", _f),
         ("w_packed", _vp), ("bias", _vp), ("y", _vp), ("stats", _vp), ("ymax", _vp), ("ymin", _vp),
         ("group", _i), ("extrema_atomic", _i), ("precision", _i),
+        ("edge_x", _vp), ("edge_stride", ctypes.c_longlong * 3), ("edge_C", _i),
+        ("in_act", _i), ("in_act_slope", _f), ("cloud_bias", _vp),
     ]
 
 
@@ -85,6 +88,7 @@ class PwApply(ctypes.Structure):
         ("stats", _vp), ("stat_rows", ctypes.c_longlong),
         ("gamma", _vp), ("beta", _vp), ("running_mean", _vp), ("running_var", _vp),
         ("eps", _f), ("momentum", _f),
+        ("act", _i), ("act_slope", _f),
     ]
 
 

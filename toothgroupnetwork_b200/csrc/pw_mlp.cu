@@ -15,6 +15,8 @@
 //   * layer 0 of a set abstraction builds its operand straight from the neighbourhood gather
 //     ([feats | xyz - centre] or [xyz - centre | feats]); layer 0 of a feature propagation reads up to two strided
 //     segments (skip features channel-first, interpolated features point-major): no grouped tensor, no concat;
+//     layer 0 of a DGCNN EdgeConv builds [x_j - x_i | x_i] from the neighbour index and the strided features (mode 2);
+//   * the activation after BatchNorm is ReLU, or LeakyReLU (DGCNN) written as torch writes it: v > 0 ? v : v * slope;
 //   * the GEMM runs TRANSPOSED (weights = M side, rows = N side); after the K loop the accumulators are staged
 //     channel-major in shared memory, so that in the epilogue a thread owns one output channel: the per-channel
 //     sum / sum^2 (fp64 atomics, two per channel per CTA), and for the last set-abstraction layer the
@@ -119,6 +121,8 @@ __device__ __forceinline__ float4 bn_scale_shift(int mode, int c, int cn, const 
     return a;
 }
 __device__ __forceinline__ float bn_apply(float x, const float4& a) { return fmaf((x - a.x) - a.y, a.z, a.w); }
+// torch's leaky_relu kernel: keeps the sign of a zero, and NaN stays NaN
+__device__ __forceinline__ float leaky_relu(float v, float slope) { return v > 0.f ? v : v * slope; }
 // torch's training-mode side effect: running = (1-m) running + m batch (variance unbiased)
 __device__ __forceinline__ void bn_update_running(int c, int cn, const double* stats, double count, float momentum, float* rmean, float* rvar)
 {
@@ -166,7 +170,8 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
         const bool valid = r < L.rows;
         // source addressing of this row
         const float* seg0 = nullptr; const float* seg1 = nullptr;   // mode 0
-        const float* pf = nullptr;                                    // mode 1: gathered feature row
+        const float* pf = nullptr;                                    // mode 1: gathered feature row; mode 2: neighbour's features
+        const float* pe = nullptr;                                    // mode 2: the centre point's features
         float rel0 = 0.f, rel1 = 0.f, rel2 = 0.f;
         bool row_ok = valid;
         if (L.mode == 0) {
@@ -174,6 +179,19 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
                 const int b = r / L.rows_per_batch, n = r - b * L.rows_per_batch;
                 seg0 = L.seg_ptr[0] + b * L.seg_batch_stride[0] + n * L.seg_row_stride[0];
                 if (L.seg_channels[1] > 0) seg1 = L.seg_ptr[1] + b * L.seg_batch_stride[1] + n * L.seg_row_stride[1];
+            }
+        } else if (L.mode == 2) {
+            if (valid) {
+                const int pt = r / L.K;                                   // b*N + n
+                const int b = pt / L.N, n = pt - b * L.N;
+                const int m = __ldg(L.gidx + r);
+                if (m >= 0 && m < L.N) {
+                    const float* xb = L.edge_x + b * L.edge_stride[0];
+                    pe = xb + n * L.edge_stride[2];
+                    pf = xb + m * L.edge_stride[2];
+                } else {
+                    row_ok = false;
+                }
             }
         } else if (valid) {
             const int grp = r / L.K;                                  // (b*S + s)
@@ -219,6 +237,16 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
                     else if (k < L.cin) v = __ldg(seg1 + (k - c0seg) * cs1);
                     x[i] = v;
                 }
+            } else if (L.mode == 2) {
+                // channel order of cat((feature - x, x), dim=3).permute(0, 3, 1, 2) (dgcnn.py:39)
+#pragma unroll
+                for (int i = 0; i < kKC; ++i) {
+                    const int k = k0 + i;
+                    float v = 0.f;
+                    if (k < L.edge_C) v = __fsub_rn(__ldg(pf + k * L.edge_stride[1]), __ldg(pe + k * L.edge_stride[1]));
+                    else if (k < L.cin) v = __ldg(pe + (k - L.edge_C) * L.edge_stride[1]);
+                    x[i] = v;
+                }
             } else {
 #pragma unroll
                 for (int i = 0; i < kKC; ++i) {
@@ -237,7 +265,8 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
                 for (int i = 0; i < kKC; ++i) {
                     const int k = k0 + i;
                     if (k < L.cin) {
-                        x[i] = fmaxf(bn_apply(x[i], affine[k]), 0.f);
+                        const float v = bn_apply(x[i], affine[k]);
+                        x[i] = L.in_act == 1 ? leaky_relu(v, L.in_act_slope) : fmaxf(v, 0.f);
                     }
                 }
             }
@@ -316,7 +345,8 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
             float f1 = 0.f, f2 = 0.f;
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
-                const float y = __uint_as_float(v[i]) + bias;
+                float y = __uint_as_float(v[i]) + bias;
+                if (L.cloud_bias && c_ok && i < nvalid) y += __ldg(L.cloud_bias + static_cast<size_t>((rb + i) / L.rows_per_batch) * L.cout + c);
                 v[i] = __float_as_uint(y);
                 if (i < nvalid) { f1 += y; f2 = fmaf(y, y, f2); }
             }
@@ -385,7 +415,8 @@ __global__ void pw_pack_weights_kernel(int cout, int cin, int nkc, const float* 
     }
 }
 
-// out[b, c_off + c, n] = relu?(scale_c * v + shift_c), v = Y[c, b*rpb + n] or the max / min pick by sign(scale)
+// out[b, c_off + c, n] = act(scale_c * v + shift_c), v = Y[c, b*rpb + n] or the max / min pick by sign(scale): BatchNorm and
+// the activation are both monotone, so the extreme that maps to the largest output is the max when scale >= 0, else the min
 __global__ void pw_apply_kernel(const tgn_pw_apply_t p)
 {
     __shared__ float4 ss;
@@ -403,9 +434,26 @@ __global__ void pw_apply_kernel(const tgn_pw_apply_t p)
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < p.rows; i += gridDim.x * blockDim.x) {
         const int b = i / p.rows_per_batch, n = i - b * p.rows_per_batch;
         float v = bn_apply(src[static_cast<size_t>(c) * p.rows + i], aff);
-        if (p.relu) v = fmaxf(v, 0.f);
+        if (p.act == 1) v = leaky_relu(v, p.act_slope);
+        else if (p.relu) v = fmaxf(v, 0.f);
         p.out[(static_cast<size_t>(b) * p.out_channels + p.out_c_offset + c) * p.rows_per_batch + n] = v;
     }
+}
+
+// out[b, c] = sum_k w[c, k] * g[b, k], accumulated in fp64 in index order and rounded once: one warp per output
+__global__ void pw_cloud_bias_kernel(int B, int cout, int cin, const float* __restrict__ w, long long w_row_stride,
+                                     const float* __restrict__ g, long long g_batch_stride, float* __restrict__ out)
+{
+    const int o = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (o >= B * cout) return;
+    const int b = o / cout, c = o - b * cout;
+    const float* wr = w + c * w_row_stride;
+    const float* gr = g + b * g_batch_stride;
+    double acc = 0.0;
+    for (int k = lane; k < cin; k += 32) acc = fma(static_cast<double>(__ldg(wr + k)), static_cast<double>(__ldg(gr + k)), acc);
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, d);
+    if (lane == 0) out[o] = static_cast<float>(acc);
 }
 
 __global__ void pw_fill_kernel(float* p, size_t n, float v)
@@ -452,7 +500,14 @@ int tgn_pw_layer_forward(const tgn_pw_layer_t* layer, void* stream)
         if (!L.xyz || !L.new_xyz || !L.gidx || L.K < 1 || L.S < 1 || L.cin != L.D + 3 || (L.D > 0 && !L.feats)) {
             set_error("pw_layer_forward: bad gather arguments"); return TGN_ERR_INVALID;
         }
+    } else if (L.mode == 2) {
+        if (!L.edge_x || !L.gidx || L.K < 1 || L.N < 1 || L.edge_C < 1 || L.cin != 2 * L.edge_C ||
+            L.rows % (static_cast<long long>(L.N) * L.K) != 0) {
+            set_error("pw_layer_forward: bad edge-feature arguments (need edge_x, gidx, K, N >= 1, cin = 2 * edge_C, rows %% (N * K) == 0)");
+            return TGN_ERR_INVALID;
+        }
     } else { set_error("pw_layer_forward: unknown mode %d", L.mode); return TGN_ERR_INVALID; }
+    if (L.cloud_bias && L.rows_per_batch < 1) { set_error("pw_layer_forward: cloud_bias needs rows_per_batch"); return TGN_ERR_INVALID; }
     if (L.in_affine == 1 && !L.in_stats) { set_error("pw_layer_forward: in_affine=1 needs in_stats"); return TGN_ERR_INVALID; }
     if (L.in_affine == 2 && (!L.in_running_mean || !L.in_running_var)) { set_error("pw_layer_forward: in_affine=2 needs running statistics"); return TGN_ERR_INVALID; }
     if (L.ymax) {
@@ -482,6 +537,18 @@ int tgn_pw_apply(const tgn_pw_apply_t* p, void* stream)
     dim3 grid(bx, p->channels);
     pw_apply_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(*p);
     return check_launch("pw_apply_kernel");
+}
+
+int tgn_pw_cloud_bias(int B, int cout, int cin, const float* w, long long w_row_stride, const float* g, long long g_batch_stride,
+                      float* out, void* stream)
+{
+    using namespace tgn;
+    if (B < 1 || cout < 1 || cin < 1 || !w || !g || !out || w_row_stride < cin || g_batch_stride < 0) {
+        set_error("pw_cloud_bias: bad arguments"); return TGN_ERR_INVALID;
+    }
+    const int outputs = B * cout;
+    pw_cloud_bias_kernel<<<(outputs + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(B, cout, cin, w, w_row_stride, g, g_batch_stride, out);
+    return check_launch("pw_cloud_bias_kernel");
 }
 
 int tgn_pw_fill(float* ptr, long long n, float value, void* stream)

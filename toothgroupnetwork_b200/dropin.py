@@ -115,6 +115,17 @@ def accelerate_dgcnn(module=None) -> None:
     dgcnn.accelerate(module)
 
 
+def accelerate_dgcnn_forward(module=None) -> None:
+    """Optional: run the no-grad forward of the DGCNN model (``DGCnnModule.forward``, models/modules/dgcnn.py:96-134) on the
+    tensor-core layer chain of ``toothgroupnetwork_b200.dgcnn``: the EdgeConv gathers, BatchNorm, LeakyReLU and the neighbour max
+    without the (B, 2C, N, k) tensors.  Under autograd the reference's own forward runs.  Imports ``models.modules.dgcnn`` from
+    ``sys.path`` when no module is passed."""
+    from . import dgcnn
+    if module is None:
+        module = importlib.import_module("models.modules.dgcnn")
+    dgcnn.accelerate_forward(module)
+
+
 def uninstall() -> None:
     for alias in _TARGETS:
         sys.modules.pop(alias, None)

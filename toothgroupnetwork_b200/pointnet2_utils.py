@@ -473,10 +473,11 @@ class _PwChain:
         desc.in_update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
 
     def run(self, convs, bns, first: "L.PwLayer", rows: int, out: torch.Tensor, out_c_offset: int, rows_per_batch_out: int,
-            group: int = 0) -> None:
+            group: int = 0, slopes: Optional[Sequence[float]] = None) -> None:
         """``first`` describes the operand source of layer 0 (mode / segments / gather fields filled by the
         caller).  group > 0: the last layer reduces max/min over ``group`` consecutive rows (set abstraction)
-        and ``out`` is (B, C_total, rows/group/B...); group == 0: ``out`` receives every row (feature propagation)."""
+        and ``out`` is (B, C_total, rows/group/B...); group == 0: ``out`` receives every row (feature propagation).
+        ``slopes``: LeakyReLU(slopes[l]) follows BatchNorm l instead of ReLU (DGCNN); None leaves every ReLU launch as it was."""
         dev = out.device
         n = len(convs)
         couts = [c.weight.shape[0] for c in convs]
@@ -496,6 +497,8 @@ class _PwChain:
                 d.seg_batch_stride[0], d.seg_row_stride[0], d.seg_chan_stride[0] = 0, 1, rows
                 d.seg_channels[1] = 0
                 self._fill_in_bn(d, bns[l - 1], stats[l - 1])
+                if slopes is not None:
+                    d.in_act, d.in_act_slope = 1, float(slopes[l - 1])
             packed = self.packed(conv)
             self.wait_packed(conv)
             d.w_packed = L.ptr(packed)
@@ -533,6 +536,8 @@ class _PwChain:
         a.running_mean, a.running_var = L.ptr(bn.running_mean), L.ptr(bn.running_var)
         a.eps, a.momentum = float(bn.eps), float(bn.momentum if bn.momentum is not None else 0.0)
         a.update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
+        if slopes is not None:
+            a.act, a.act_slope = 1, float(slopes[-1])
         L.call("tgn_pw_apply", ctypes.byref(a), st)
         for b in bns:
             if b.training and b.num_batches_tracked is not None:
