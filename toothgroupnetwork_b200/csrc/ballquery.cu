@@ -24,26 +24,7 @@ namespace {
 
 constexpr int kTile = 1024;   // points staged per shared-memory tile (16 KB as SoA x,y,z,|p|^2)
 
-// |p|^2 as torch.sum(p ** 2, -1) rounds it ON THE GPU (square_distance :39-40), measured with torch 2.11
-// (scripts/diag_sumsq.py): a strided reduction (the permuted views the reference's modules
-// pass) accumulates in index order, (x*x + y*y) + z*z -- the same as torch on the CPU; a CONTIGUOUS (..., 3) tensor
-// (e.g. new_xyz fresh out of index_points) goes through the vectorised reduce path and comes out as
-// (x*x + z*z) + y*y.  `alt` selects the second form; the Python layer derives it from the layout the reference's
-// own call would see, per operand.
-__device__ __forceinline__ float sq_norm_unfused(float x, float y, float z, bool alt) {
-    return alt ? __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(z, z)), __fmul_rn(y, y))
-               : __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
-}
-__device__ __forceinline__ float sq_dist_expanded(float ax, float ay, float az, float an, float bx, float by, float bz,
-                                                  float bn) {
-    float dot = __fmul_rn(ax, bx);
-    dot = __fmaf_rn(ay, by, dot);
-    dot = __fmaf_rn(az, bz, dot);
-    float d = __fmul_rn(-2.0f, dot);
-    d = __fadd_rn(d, an);
-    return __fadd_rn(d, bn);
-}
-
+// sq_norm_unfused / sq_dist_expanded (ballquery.cuh) round as the reference's square_distance does.
 // The same when the reference's matmul has a single column (one dst point per batch, tsegnet.get_ddf): cuBLAS on H100 then
 // takes a matrix-vector path that rounds the dot product as fma(ay, by, ax*bx) + az*bz (measured with torch 2.11 / cuBLAS
 // for CUDA 12.8; two or more columns round as the fused chain above).
@@ -346,9 +327,7 @@ int tgn_ball_query(int B, int N, int S, float r2, int nsample, const float* xyz,
         BqGridWs ws{};
         const size_t bytes = bq_grid_workspace_bytes(B, N, &ws);
         if (cudaMallocAsync(reinterpret_cast<void**>(&grid_ws), bytes, st) == cudaSuccess) {
-            ws.ga = reinterpret_cast<float4*>(grid_ws + reinterpret_cast<size_t>(ws.ga));
-            ws.gb = reinterpret_cast<float4*>(grid_ws + reinterpret_cast<size_t>(ws.gb));
-            ws.gj = reinterpret_cast<int2*>(grid_ws + reinterpret_cast<size_t>(ws.gj));
+            ws.rec = reinterpret_cast<float4*>(grid_ws + reinterpret_cast<size_t>(ws.rec));
             ws.cell_start = reinterpret_cast<int*>(grid_ws + reinterpret_cast<size_t>(ws.cell_start));
             ws.org = reinterpret_cast<float4*>(grid_ws + reinterpret_cast<size_t>(ws.org));
             ws.dim = reinterpret_cast<int4*>(grid_ws + reinterpret_cast<size_t>(ws.dim));
