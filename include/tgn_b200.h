@@ -105,6 +105,19 @@ size_t tgn_dbscan_bytes(int n);
 int tgn_dbscan(int n, const float *xyz, double eps, int min_samples, void *workspace, int *labels, unsigned char *core, int *n_clusters,
                void *stream);
 
+/* scikit-learn 1.9's KMeans(k, init="k-means++", n_init=1, algorithm="lloyd", max_iter).fit on float32 (n,3) points, one fit per
+ * CTA (ops_utils.clustering_points(method="kmeans")).  B fits of points X (N,3) float32 DEVICE, fit f holding rows offsets[f] ..
+ * offsets[f+1]-1 (offsets (B+1) int32 DEVICE), already centred by the host (X - X.mean(0)); 1 <= k <= 64 and k <= each fit's n.
+ * Per fit, DEVICE: first (B) int32 = random_state.choice(n, p=w/w.sum()); uniforms (B, k-1, 2+int(log k)) float64 =
+ * random_state.uniform draws; tol (B) float32 = mean(var(X)) * tol.  Workspace of tgn_kmeans_bytes(N, B) DEVICE bytes.
+ * Outputs, DEVICE: labels (N) int32, init (B,k) int64 (the k-means++ indices), centers (B,k,3) float32 (centred), n_iter (B),
+ * inertia (B) float32, relocated (B) int32 = 1 when a cluster emptied (scikit-learn relocates it; not restated, the other
+ * outputs of that fit are then meaningless). */
+size_t tgn_kmeans_bytes(long long n_total, int B);
+int tgn_kmeans(int B, long long n_total, int k, int max_iter, const int *offsets, const float *X, const int *first, const double *uniforms,
+               const float *tol, void *workspace, int *labels, long long *init, float *centers, int *n_iter, float *inertia, int *relocated,
+               void *stream);
+
 /* Exact float64 kNN with a fused label vote: the answer of sklearn KDTree(xyz).query(queries, k) -- boundary detection of
  * InferencePipeLine.get_boundary_sampled_feats (inference_pipeline_tgn.py:289-330).  xyz (n,3) and queries (m,3) float64
  * DEVICE; 1 <= k <= 64, k <= n.  Distances d2 = (dx*dx + dy*dy) + dz*dz in float64 without contraction, neighbours ascending

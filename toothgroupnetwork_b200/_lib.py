@@ -57,6 +57,7 @@ _SIGS = {
     "tgn_pw_apply": [_vp, _vp],
     "tgn_pw_fill": [_vp, ctypes.c_longlong, _f, _vp],
     "tgn_pw_cloud_bias": [_i, _i, _i, _vp, ctypes.c_longlong, _vp, ctypes.c_longlong, _vp, _vp],
+    "tgn_kmeans": [_i, ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
 }
 
 
@@ -116,7 +117,7 @@ REFERENCE_LAUNCHERS = [
     "subtraction_forward_cuda_launcher", "subtraction_backward_cuda_launcher",
     "aggregation_forward_cuda_launcher", "aggregation_backward_cuda_launcher",
 ]
-EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes"]
+EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes"]
 
 
 class TgnError(RuntimeError):
@@ -150,6 +151,8 @@ def load() -> ctypes.CDLL:
     lib.tgn_dbscan_bytes.restype = ctypes.c_size_t
     lib.tgn_knn_f64_bytes.argtypes = [_i]
     lib.tgn_knn_f64_bytes.restype = ctypes.c_size_t
+    lib.tgn_kmeans_bytes.argtypes = [ctypes.c_longlong, _i]
+    lib.tgn_kmeans_bytes.restype = ctypes.c_size_t
     lib.tgn_pw_struct_size.argtypes = [_i]
     lib.tgn_pw_struct_size.restype = _i
     lib.tgn_pt_layer_struct_size.restype = _i

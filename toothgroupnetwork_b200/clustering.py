@@ -173,3 +173,135 @@ def accelerate_dbscan(module) -> None:
     inference_pipelines/inference_pipeline_tsegnet.py) at the device implementation."""
     if hasattr(module, "DBSCAN"):
         module.DBSCAN = DBSCAN
+
+
+_KMEANS_MAX_K = 64
+
+
+def kmeans_device(X: torch.Tensor, offsets: torch.Tensor, k: int, first: torch.Tensor, uniforms: torch.Tensor, tol: torch.Tensor,
+                  max_iter: int = 300):
+    """A batch of k-means++ / Lloyd fits on csrc/kmeans.cu, one CTA each.  X (N,3) float32 CUDA, the fits' points already
+    centred, fit f at rows offsets[f]:offsets[f+1] (int32, B+1); first (B) int32, uniforms (B, k-1, 2+int(log k)) float64 and tol
+    (B) float32 as ``KMeans.fit`` draws and computes them.  Returns (labels (N) int32, init (B,k) int64, centres (B,k,3) float32
+    centred, n_iter (B) int32, inertia (B) float32, relocated (B) int32), all on the device."""
+    L.require_cuda(X, offsets, first, uniforms, tol)
+    B = offsets.numel() - 1
+    N = X.shape[0]
+    if X.dim() != 2 or X.shape[1] != 3 or X.dtype != torch.float32:
+        raise L.TgnError(f"kmeans expects (n,3) float32 points, got {tuple(X.shape)} {X.dtype}")
+    if not 1 <= k <= _KMEANS_MAX_K:
+        raise L.TgnError(f"kmeans: 1 <= n_clusters <= {_KMEANS_MAX_K} is implemented, got {k}")
+    dev = X.device
+    X, offsets, first, tol = X.contiguous(), offsets.int().contiguous(), first.int().contiguous(), tol.float().contiguous()
+    uniforms = uniforms.double().contiguous()
+    labels = torch.empty(N, dtype=torch.int32, device=dev)
+    init = torch.empty(B, k, dtype=torch.int64, device=dev)
+    centres = torch.empty(B, k, 3, dtype=torch.float32, device=dev)
+    n_iter = torch.empty(B, dtype=torch.int32, device=dev)
+    inertia = torch.empty(B, dtype=torch.float32, device=dev)
+    relocated = torch.empty(B, dtype=torch.int32, device=dev)
+    if B:
+        ws = torch.empty(int(L.load().tgn_kmeans_bytes(N, B)), dtype=torch.uint8, device=dev)
+        L.call("tgn_kmeans", B, N, int(k), int(max_iter), L.ptr(offsets), L.ptr(X), L.ptr(first), L.ptr(uniforms) if k > 1 else None,
+               L.ptr(tol), L.ptr(ws), L.ptr(labels), L.ptr(init), L.ptr(centres), L.ptr(n_iter), L.ptr(inertia), L.ptr(relocated),
+               L.stream_ptr())
+    return labels, init, centres, n_iter, inertia, relocated
+
+
+def _random_state(seed) -> np.random.RandomState:
+    """sklearn.utils.check_random_state: numpy's global generator for None, a new one for an int, the instance itself"""
+    if seed is None or seed is np.random:
+        return np.random.mtrand._rand
+    if isinstance(seed, (int, np.integer)):
+        return np.random.RandomState(seed)
+    if isinstance(seed, np.random.RandomState):
+        return seed
+    raise ValueError(f"{seed!r} cannot be used to seed a numpy.random.RandomState instance")
+
+
+def kmeans_prepare(X: np.ndarray, k: int, tol: float, rs: np.random.RandomState):
+    """What ``KMeans.fit`` computes on the host before its k-means++ seeding, with the same numpy calls on the same arrays, and
+    the draws of ``_kmeans_plusplus`` on ``rs``: (X - X.mean(0) float32, X.mean(0), float32 tolerance, first index,
+    (k-1, 2 + int(log k)) float64 uniforms).  The draws do not depend on the data, so ``rs`` ends where scikit-learn leaves it."""
+    X = np.array(X, dtype=np.float32, order="C", copy=True)
+    n = X.shape[0]
+    sw = np.ones(n, dtype=np.float32)
+    tol = np.float32(np.mean(np.var(X, axis=0)) * tol if tol != 0 else 0)
+    x_mean = X.mean(axis=0)
+    X -= x_mean
+    trials = 2 + int(np.log(k))
+    first = int(rs.choice(n, p=sw / sw.sum()))
+    u = np.stack([rs.uniform(size=trials) for _ in range(k - 1)]) if k > 1 else np.zeros((0, trials))
+    return X, x_mean, tol, first, u
+
+
+class KMeans:
+    """The slice of ``sklearn.cluster.KMeans`` the reference uses -- ``KMeans(k, init="k-means++").fit(points)`` then
+    ``.labels_`` / ``.cluster_centers_`` / ``.inertia_`` / ``.n_iter_`` (ops_utils.py:32 in ``clustering_points`` and
+    ``find_k_kmeans``) -- on csrc/kmeans.cu, on float32 (n, 3) points.
+
+    The host makes exactly scikit-learn's numpy calls (tolerance, mean, the generator draws of k-means++ on the generator
+    ``check_random_state(random_state)`` returns, so the global one for ``random_state=None``) and the device does the rest with
+    single-threaded scikit-learn's float32 rounding: labels, centres and ``n_iter_`` equal its own.  A fit in which a cluster
+    empties is redone by scikit-learn itself from the generator state saved before the draws; ``host_fits`` counts those."""
+
+    host_fits = 0
+
+    def __init__(self, n_clusters: int = 8, *, init="k-means++", n_init="auto", max_iter: int = 300, tol: float = 1e-4,
+                 verbose: int = 0, random_state=None, copy_x: bool = True, algorithm: str = "lloyd"):
+        if (not isinstance(init, str) or init != "k-means++" or n_init not in ("auto", 1) or algorithm != "lloyd" or verbose
+                or copy_x is not True):
+            raise L.TgnError(f"KMeans: only init='k-means++', n_init='auto' or 1, algorithm='lloyd', verbose=0, copy_x=True is "
+                             f"implemented (got init={init!r}, n_init={n_init!r}, algorithm={algorithm!r}, verbose={verbose!r}, "
+                             f"copy_x={copy_x!r})")
+        self.n_clusters, self.init, self.n_init, self.max_iter, self.tol = int(n_clusters), init, n_init, int(max_iter), tol
+        self.verbose, self.random_state, self.copy_x, self.algorithm = verbose, random_state, copy_x, algorithm
+
+    def fit(self, X, y=None, sample_weight=None):
+        if sample_weight is not None:
+            raise L.TgnError("KMeans: sample_weight is not implemented")
+        X = X.detach().cpu().numpy() if isinstance(X, torch.Tensor) else np.asarray(X)
+        if X.dtype != np.float32 or X.ndim != 2 or X.shape[1] != 3:
+            raise L.TgnError(f"KMeans: expected (n, 3) float32 points, got {X.shape} {X.dtype}")
+        if not np.isfinite(X).all():
+            raise ValueError("Input X contains NaN or infinity.")
+        n, k = X.shape[0], self.n_clusters
+        if n < k:
+            raise ValueError(f"n_samples={n} should be >= n_clusters={k}.")
+        if not 1 <= k <= _KMEANS_MAX_K:
+            raise L.TgnError(f"KMeans: 1 <= n_clusters <= {_KMEANS_MAX_K} is implemented, got {k}")
+        if not torch.cuda.is_available():
+            raise L.TgnError("KMeans needs a CUDA device (there is no CPU path)")
+        rs = _random_state(self.random_state)
+        saved = rs.get_state()
+        X0 = X
+        X, x_mean, tol, first, u = kmeans_prepare(X, k, self.tol, rs)
+        trials = u.shape[1]
+        host = [np.array([0, n], np.int32), np.array([first], np.int32), np.array([tol], np.float32)]
+        dev = [torch.from_numpy(a).cuda() for a in host]
+        labels, init, centres, n_iter, inertia, relocated = kmeans_device(
+            torch.from_numpy(X).cuda(), dev[0], k, dev[1], torch.from_numpy(u.reshape(1, k - 1, trials)).cuda(), dev[2], self.max_iter)
+        small = torch.cat([n_iter.double(), inertia.double(), relocated.double()]).cpu().numpy()
+        if small[2]:
+            from sklearn.cluster import KMeans as SkKMeans
+            type(self).host_fits += 1
+            rs.set_state(saved)
+            ref = SkKMeans(k, init="k-means++", n_init=1, max_iter=self.max_iter, tol=self.tol, random_state=rs).fit(X0)
+            self.labels_, self.cluster_centers_ = ref.labels_, ref.cluster_centers_
+            self.inertia_, self.n_iter_ = ref.inertia_, ref.n_iter_
+        else:
+            self.labels_ = labels.cpu().numpy()
+            self.cluster_centers_ = centres[0].cpu().numpy() + x_mean
+            self.inertia_, self.n_iter_ = float(np.float32(small[1])), int(small[0])
+            self.init_indices_ = init[0].cpu().numpy()
+        self.n_features_in_ = 3
+        return self
+
+    def fit_predict(self, X, y=None, sample_weight=None):
+        return self.fit(X, y, sample_weight).labels_
+
+
+def accelerate_kmeans(module) -> None:
+    """Point a module's ``KMeans`` name (``from sklearn.cluster import KMeans`` in ops_utils.py) at the device implementation."""
+    if hasattr(module, "KMeans"):
+        module.KMeans = KMeans

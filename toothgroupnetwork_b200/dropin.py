@@ -67,6 +67,16 @@ def accelerate_ops_utils(ops_utils_module=None) -> None:
             clustering.accelerate_dbscan(sys.modules[name])
 
 
+def accelerate_kmeans(module=None) -> None:
+    """Optional: point the ``KMeans`` name of the reference's ``ops_utils`` (``clustering_points(method="kmeans")`` and
+    ``find_k_kmeans``, ops_utils.py:32) at ``toothgroupnetwork_b200.clustering.KMeans``, which fits on the GPU with scikit-learn's
+    labels.  Imports ``ops_utils`` from ``sys.path`` when no module is passed."""
+    from . import clustering
+    if module is None:
+        module = importlib.import_module("ops_utils")
+    clustering.accelerate_kmeans(module)
+
+
 def accelerate_blocks(blocks_module=None) -> None:
     """Optional: run the no-grad forwards of the reference's ``PointTransformerLayer`` / ``TransitionDown``
     (models/modules/cbl_point_transformer/blocks.py:31-44, :59-79) on the fused kernels of
