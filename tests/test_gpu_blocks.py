@@ -84,6 +84,17 @@ def schedule(request):
 @pytest.mark.parametrize("c,K,n", [(32, 36, 6000), (64, 7, 777), (128, 24, 1500), (256, 24, 400), (512, 24, 93)])
 @pytest.mark.parametrize("train_bn", [True, False])
 def test_fused_layer_against_oracle_float64(c, K, n, train_bn, schedule):
+    _layer_against_oracle(c, K, n, train_bn, offset=0.0)
+
+
+@pytest.mark.parametrize("c,K,n", [(32, 36, 6000), (128, 24, 1500)])
+def test_fused_layer_offset_channels_against_oracle_float64(c, K, n, schedule):
+    """linear_k.bias + 100 on every fourth channel: BatchNorm_a sees |mean| / std ~ 100 there, and its batch variance must
+    survive the offset"""
+    _layer_against_oracle(c, K, n, True, offset=100.0)
+
+
+def _layer_against_oracle(c, K, n, train_bn, offset):
     torch.manual_seed(c)
     layer = Layer(c, K).train(train_bn)
     g = torch.Generator().manual_seed(1)
@@ -94,6 +105,8 @@ def test_fused_layer_against_oracle_float64(c, K, n, train_bn, schedule):
                 m.bias.copy_(torch.randn(m.bias.shape, generator=g) * 0.1)
                 m.running_mean.copy_(torch.randn(m.running_mean.shape, generator=g) * 0.1)
                 m.running_var.copy_(torch.rand(m.running_var.shape, generator=g) + 0.5)
+    with torch.no_grad():
+        layer.linear_k.bias[0::4] += offset
     state = {k: v.clone() for k, v in layer.state_dict().items()}
     p = clouds.dental_arch(n, 4)[0].contiguous()
     x = torch.randn(n, c, generator=g)

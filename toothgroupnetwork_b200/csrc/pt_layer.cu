@@ -125,11 +125,6 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
 #pragma unroll
             for (int q = 0; q < CPL; ++q) xq[q] = __ldg(L.xq + static_cast<size_t>(i) * C + 32 * q + lane);
         }
-        float f1[PASS == 1 ? CPL : 1], f2[PASS == 1 ? CPL : 1];
-        if (PASS == 1) {
-#pragma unroll
-            for (int q = 0; q < CPL; ++q) { f1[q] = 0.f; f2[q] = 0.f; }
-        }
         float out[PASS == 3 ? CPL : 1];
 
         for (int phase = 0; phase < (PASS == 3 ? 2 : 1); ++phase) {
@@ -180,8 +175,9 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
 #pragma unroll
                 for (int q = 0; q < CPL; ++q) w0[q] = (__ldg(L.xk + static_cast<size_t>(nbr) * C + 32 * q + lane) - xq[q]) + pr[q];
                 if (PASS == 1) {
+                    // fp64 per element, as passes 0 and 2: fp32 partial sums of w0^2 lose the variance of a channel whose |mean| >> std
 #pragma unroll
-                    for (int q = 0; q < CPL; ++q) { f1[q] += w0[q]; f2[q] = fmaf(w0[q], w0[q], f2[q]); }
+                    for (int q = 0; q < CPL; ++q) { acc1[q] += w0[q]; acc2[q] = fma(static_cast<double>(w0[q]), static_cast<double>(w0[q]), acc2[q]); }
                     continue;
                 }
                 // c -> c/8: per-lane partial sums over this lane's channels, butterfly, every lane holds all CS values
@@ -215,10 +211,6 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
                     logits[j * CS + mo] = s;
                 }
             }
-        }
-        if (PASS == 1) {
-#pragma unroll
-            for (int q = 0; q < CPL; ++q) { acc1[q] += f1[q]; acc2[q] += f2[q]; }
         }
         if (PASS == 3 && !CTAQ) {
 #pragma unroll

@@ -90,12 +90,14 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// ordered by the sign BIT, not by v >= 0: -0.0 compares >= 0 but its bits are INT_MIN as a signed int, so it belongs on the
+// unsigned side with the other negative values (where it is the largest)
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-    if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+    if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 __device__ __forceinline__ void atomic_min_float(float* addr, float v) {
-    if (v >= 0.f) atomicMin(reinterpret_cast<int*>(addr), __float_as_int(v));
+    if (__float_as_int(v) >= 0) atomicMin(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMax(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
@@ -342,16 +344,20 @@ __global__ void __launch_bounds__(kThreads, 1) pw_layer_kernel(const PwArgs a)
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(trow[cb + i]);
             const int nvalid = min(32, L.rows - rb);
-            float f1 = 0.f, f2 = 0.f;
+            // the block's fp32 partial sums are taken about its first value p (row rb is always valid) and re-expanded in fp64:
+            // sum (y - p)^2 keeps the variance of a channel whose |mean| >> std, which sum y^2 in fp32 would round away
+            float p = 0.f, f1 = 0.f, f2 = 0.f;
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
                 float y = __uint_as_float(v[i]) + bias;
                 if (L.cloud_bias && c_ok && i < nvalid) y += __ldg(L.cloud_bias + static_cast<size_t>((rb + i) / L.rows_per_batch) * L.cout + c);
                 v[i] = __float_as_uint(y);
-                if (i < nvalid) { f1 += y; f2 = fmaf(y, y, f2); }
+                if (i == 0) p = y;
+                if (i < nvalid) { const float d = __fsub_rn(y, p); f1 += d; f2 = fmaf(d, d, f2); }
             }
-            s1 += static_cast<double>(f1);
-            s2 += static_cast<double>(f2);
+            const double pd = static_cast<double>(p), np = static_cast<double>(nvalid) * pd;
+            s1 += np + static_cast<double>(f1);
+            s2 += fma(pd, np + 2.0 * static_cast<double>(f1), static_cast<double>(f2));
             if (L.y && c_ok) {
                 float* dst = L.y + static_cast<size_t>(c) * L.rows + rb;
                 if (vec_ok && nvalid == 32) {
