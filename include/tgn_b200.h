@@ -234,12 +234,15 @@ int tgn_transpose_cn(int B, int C, int N, const float *in, float *out, void *str
  * folded into weight/bias by the caller).
  *   xyz (B,N,3); feats (B,N,D) point-major or NULL (D = 0); new_xyz (B,S,3); group_idx (B,S,K) int32
  *   xyz_first: 1 -> channels [xyz_rel, feats] (SSG, :169), 0 -> [feats, xyz_rel] (MSG, :285)
+ *   a group_idx entry outside [0, N) (the ball query's N for an empty ball) is an all-zero operand row
  *   n_layers in [1,4]; channels[n_layers+1] HOST array, channels[0] = 3 + D; every width <= 128
  *   weights[l] (C_{l+1}, C_l) row-major DEVICE, biases[l] (C_{l+1}) DEVICE; the two pointer arrays are HOST arrays
  *   out: channel-first (B, out_c_total, S); this branch writes channels [out_c_offset, +C_last)
  *   engine: 0 = auto (2 when the shape fits it, else 3, else 1), 1 = fp32 CUDA-core kernel (exact FMA),
- *           2 = tensor-core (wgmma) 3xTF32 kernel (widths <= 64, any K <= 128, ~2^-21), 3 = tensor-core kernel for wide layers
- *           (first layer 3xTF32, later layers as three bf16x2-split MMAs, ~1e-5; at least two layers, K in {16,32,64,128}),
+ *           2 = tensor-core (wgmma) 3xTF32 kernel (widths <= 64, any K <= 128, ~2^-21; operands and weights within 220 KB of
+ *           shared memory: four 64-wide layers are refused), 3 = tensor-core kernel for wide layers
+ *           (first layer 3xTF32, later layers as three bf16x2-split MMAs, ~1e-5; at least two layers, K in {16,32,64,128},
+ *           within 224 KB of shared memory: three 128-wide layers are refused),
  *           5 = engine 2 in half-size CTAs.  Any other value is refused (engine 4 was Blackwell-only and is gone). */
 int tgn_sa_group_mlp_max(int B, int N, int S, int K, int D, const float *xyz, const float *feats, const float *new_xyz,
                          const int *group_idx, int xyz_first, int n_layers, const int *channels,

@@ -259,7 +259,8 @@ def test_set_abstraction_msg_eval_matches_reference_fixture(golden_dir, engine):
 @pytest.mark.parametrize("engine", [pn2.ENGINE_AUTO, pn2.ENGINE_TCW, pn2.ENGINE_FP32])
 def test_real_pointnet_pp_sa1_shape_matches_reference_fixture(golden_dir, engine):
     """The real pointnet_pp SA1 (pointnet_pp.py:13: two 9->128->128 branches, K = 32 / 64) against a fixture made
-    by the reference's own Python (tests/golden/make_ref_torch_msg128_golden.py).  AUTO takes the wide tensor-core engine."""
+    by the reference's own Python (tests/golden/make_ref_torch_msg128_golden.py).  The module's AUTO stops the single-kernel
+    engines at 64 channels (SA_FUSED_AUTO_MAX_WIDTH), so this shape runs on the layer-per-launch chain of csrc/pw_mlp.cu."""
     fix = load(golden_dir, "ref_torch_msg128.npz")
     feats = torch.from_numpy(fix["feats"]).cuda()
     msg = pn2.PointNetSetAbstractionMsg(128, [0.05, 0.1], [32, 64], 6, [[128, 128], [128, 128]]).cuda().eval()
