@@ -173,7 +173,12 @@ int tgn_weighted_gather(int n, int c, int k, const float *input, const int *idx,
  *   tgn_weighted_gather_backward_det:  keys = idx (n,k) flattened; grad_out (n,c), weight (n,k):
  *        per i: G_i[r,:] = sum_{n ascending, idx[n,i]=r} grad_out[n,:]*weight[n,i];  grad_in = ((G_{k-1}+G_{k-2})+...)+G_0
  *        -- the order in which autograd sums the k index_put results of pointops.interpolation (pointops.py:177-179);
- *        single != 0: one accumulation over all (n,i) in ascending n*k+i -- the backward of pointnet2_utils.py:340. */
+ *        single != 0: one accumulation over all (n,i) in ascending n*k+i -- the backward of pointnet2_utils.py:340.
+ *   c == 1 follows torch's kernel for one-element slices: for a row (of each accumulation) with d terms, lane L of a warp adds
+ *        terms L, 32+L, ... below F = 32*floor(d/32), the 32 lane sums are reduced by shfl_down (16, 8, 4, 2, 1), then terms
+ *        F .. d-1 are added in order (d < 32: the plain ascending sum).  Every c > 1 is the ascending sequential sum.
+ *   Keys outside [0, n_rows) are dropped (they add to no row); a row without keys gets 0.  M == 0 is valid: tgn_csr_build writes
+ *        an empty inverse (row_start all zero) and both backwards then write zeros.  k > 8 is refused (callers use atomics). */
 size_t tgn_csr_bytes(long long M, int n_rows);
 int tgn_csr_build(long long M, int n_rows, const int *keys, void *workspace, void *stream);
 int tgn_gather_backward_det(long long M, int n_rows, int c, const void *workspace, const float *grad_out, float *grad_in, void *stream);

@@ -178,6 +178,89 @@ __global__ void __launch_bounds__(256) weighted_gather_bwd_det_kernel(int n_rows
     }
 }
 
+// c == 1: torch's index_put takes another kernel for slices of one element (indexing_backward_kernel_stride_1, ATen
+// Indexing.cu).  For a destination row with d contributions t_0 .. t_{d-1} (ascending source position) and F = 32*floor(d/32):
+// lane L sums t_L, t_{32+L}, ... below F sequentially, the 32 lane sums are reduced by shfl_down (offsets 16, 8, 4, 2, 1),
+// then lane 0 adds t_F .. t_{d-1} sequentially; d < 32 is the plain sequential sum.  One warp per row reproduces that.
+// The weighted form applies it to every index_put (each i, or all positions at once when `single`); w == nullptr is the
+// plain gather backward (term = grad_out[p]).  A row's list is walked twice in chunks of 32: once to count every index_put's
+// d, once to hand each term to the lane that adds it (through shared memory) or to lane 0's tail.
+template <int KMAX>
+__global__ void __launch_bounds__(256) gather_c1_det_kernel(int n_rows, int k, int single, const int* __restrict__ row_start,
+                                                            const int* __restrict__ order, const float* __restrict__ grad_out,
+                                                            const float* __restrict__ w, float* __restrict__ grad_in)
+{
+    __shared__ float xch_s[8][32];
+    __shared__ float tail_s[8][KMAX][32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int row = blockIdx.x * 8 + wid;
+    if (row >= n_rows) return;
+    const int nk = single ? 1 : k;
+    const int s = __ldg(row_start + row), t = __ldg(row_start + row + 1);
+    const unsigned lt = (1u << lane) - 1u;
+    int d[KMAX];
+#pragma unroll
+    for (int u = 0; u < KMAX; ++u) d[u] = 0;
+    if (nk == 1) {
+        d[0] = t - s;
+    } else {
+        for (int q0 = s; q0 < t; q0 += 32) {
+            const int q = q0 + lane;
+            const int i = q < t ? __ldg(order + q) % k : -1;
+#pragma unroll
+            for (int u = 0; u < KMAX; ++u) d[u] += __popc(__ballot_sync(FULL, i == u));
+        }
+    }
+    float acc[KMAX];
+    int cnt[KMAX];
+#pragma unroll
+    for (int u = 0; u < KMAX; ++u) { acc[u] = 0.f; cnt[u] = 0; }
+    for (int q0 = s; q0 < t; q0 += 32) {
+        const int q = q0 + lane;
+        int i = -1;
+        float term = 0.f;
+        if (q < t) {
+            const int p = __ldg(order + q);
+            if (w) {
+                const int n = p / k;
+                i = single ? 0 : p - n * k;
+                term = __fmul_rn(__ldg(grad_out + n), __ldg(w + p));
+            } else {
+                i = 0;
+                term = __ldg(grad_out + p);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < KMAX; ++u) {
+            if (u >= nk) break;
+            const unsigned mask = __ballot_sync(FULL, i == u);
+            const int full = d[u] & ~31;
+            if (i == u) {
+                const int j = cnt[u] + __popc(mask & lt);
+                if (j < full) xch_s[wid][j & 31] = term;
+                else tail_s[wid][u][j - full] = term;
+            }
+            __syncwarp();
+            const int want = cnt[u] + ((lane - cnt[u]) & 31);       // the rank this lane adds, if this chunk holds it
+            if (want < cnt[u] + __popc(mask) && want < full) acc[u] = __fadd_rn(acc[u], xch_s[wid][lane]);
+            __syncwarp();
+            cnt[u] += __popc(mask);
+        }
+    }
+    float tot = 0.f;
+#pragma unroll
+    for (int u = KMAX - 1; u >= 0; --u) {
+        if (u >= nk) continue;
+        float g = acc[u];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) g = __fadd_rn(g, __shfl_down_sync(FULL, g, off));
+        for (int j = d[u] & ~31; j < d[u]; ++j) g = __fadd_rn(g, tail_s[wid][u][j - (d[u] & ~31)]);
+        g = __fadd_rn(0.f, g);                                      // index_put adds into the zero-filled gradient
+        tot = u == nk - 1 ? g : __fadd_rn(tot, g);
+    }
+    if (lane == 0) grad_in[row] = tot;
+}
+
 int grid_for_elems(size_t n) { return static_cast<int>(std::min<size_t>((n + 255) / 256, 16 * static_cast<size_t>(sm_count()))); }
 
 }  // namespace
@@ -190,12 +273,19 @@ size_t tgn_csr_bytes(long long M, int n_rows) { return tgn::carve(M, n_rows, nul
 int tgn_csr_build(long long M, int n_rows, const int* keys, void* workspace, void* stream)
 {
     using namespace tgn;
-    if (M <= 0 || n_rows <= 0) return TGN_OK;
-    if (!keys || !workspace) { set_error("csr_build: null argument"); return TGN_ERR_INVALID; }
+    if (n_rows <= 0) return TGN_OK;
+    if (!workspace || (M > 0 && !keys)) { set_error("csr_build: null argument"); return TGN_ERR_INVALID; }
     if (M > INT_MAX) { set_error("csr_build: %lld source positions exceed int32", M); return TGN_ERR_INVALID; }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CsrWs ws{};
-    carve(M, n_rows, &ws, static_cast<unsigned char*>(workspace));
+    carve(M < 0 ? 0 : M, n_rows, &ws, static_cast<unsigned char*>(workspace));
+    if (M <= 0) {           // empty index: every row is empty, and both backwards then write zeros
+        if (cudaMemsetAsync(ws.row_start, 0, (static_cast<size_t>(n_rows) + 1) * sizeof(int), st) != cudaSuccess) {
+            set_error("csr_build: memset failed: %s", cudaGetErrorString(cudaGetLastError()));
+            return TGN_ERR_CUDA;
+        }
+        return TGN_OK;
+    }
     if (cudaMemsetAsync(ws.cursor, 0, static_cast<size_t>(n_rows) * sizeof(int), st) != cudaSuccess) {
         set_error("csr_build: memset failed: %s", cudaGetErrorString(cudaGetLastError()));
         return TGN_ERR_CUDA;
@@ -217,6 +307,11 @@ int tgn_gather_backward_det(long long M, int n_rows, int c, const void* workspac
     if (n_rows <= 0 || c <= 0) return TGN_OK;
     CsrWs ws{};
     carve(M, n_rows, &ws, const_cast<unsigned char*>(static_cast<const unsigned char*>(workspace)));
+    if (c == 1) {
+        gather_c1_det_kernel<1><<<(n_rows + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(n_rows, 1, 1, ws.row_start, ws.order,
+                                                                                                  grad_out, nullptr, grad_in);
+        return check_launch("gather_c1_det_kernel");
+    }
     gather_sum_det_kernel<<<grid_for_elems(static_cast<size_t>(n_rows) * c), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         n_rows, c, ws.row_start, ws.order, grad_out, grad_in);
     return check_launch("gather_sum_det_kernel");
@@ -232,6 +327,13 @@ int tgn_weighted_gather_backward_det(long long M, int n_rows, int c, int k, int 
     carve(M, n_rows, &ws, const_cast<unsigned char*>(static_cast<const unsigned char*>(workspace)));
     const int grid = grid_for_elems(static_cast<size_t>(n_rows) * c);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (c == 1) {
+        const int blocks = (n_rows + 7) / 8;
+        if (k <= 1 || single) gather_c1_det_kernel<1><<<blocks, 256, 0, st>>>(n_rows, k, single, ws.row_start, ws.order, grad_out, weight, grad_in);
+        else if (k <= 3) gather_c1_det_kernel<3><<<blocks, 256, 0, st>>>(n_rows, k, 0, ws.row_start, ws.order, grad_out, weight, grad_in);
+        else gather_c1_det_kernel<8><<<blocks, 256, 0, st>>>(n_rows, k, 0, ws.row_start, ws.order, grad_out, weight, grad_in);
+        return check_launch("gather_c1_det_kernel");
+    }
     if (k <= 1 || single) weighted_gather_bwd_det_kernel<1><<<grid, 256, 0, st>>>(n_rows, c, k, single, ws.row_start, ws.order, grad_out, weight, grad_in);
     else if (k <= 3) weighted_gather_bwd_det_kernel<3><<<grid, 256, 0, st>>>(n_rows, c, k, 0, ws.row_start, ws.order, grad_out, weight, grad_in);
     else weighted_gather_bwd_det_kernel<8><<<grid, 256, 0, st>>>(n_rows, c, k, 0, ws.row_start, ws.order, grad_out, weight, grad_in);
