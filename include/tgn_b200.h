@@ -118,6 +118,17 @@ int tgn_kmeans(int B, long long n_total, int k, int max_iter, const int *offsets
                const float *tol, void *workspace, int *labels, long long *init, float *centers, int *n_iter, float *inertia, int *relocated,
                void *stream);
 
+/* The seed ascent of scikit-learn 1.9's MeanShift(bandwidth, max_iter).fit on float64 (n,3) points with seeds = X: each
+ * seed's _mean_shift_single_seed, one warp per seed (the elongated-cluster split of ops_utils.get_clustering_labels).  The
+ * KD tree is scikit-learn's KDTree(X, leaf_size=30).get_arrays(), DEVICE: Xt (n,3) float64 = X[idx_array]; idx (n) int64 =
+ * idx_array; nodes (n_nodes,3) int32 = idx_start, idx_end, is_leaf; bounds (2,n_nodes,3) float64 = node_bounds.
+ * stop_thresh = 1e-3 * bandwidth as the host computes it.  Outputs by index in X, DEVICE: means (n,3) float64 (the seed's
+ * final mean), info (n,3) int32 = member count of the last query (0 when it found no point), completed iterations, and a flag
+ * (1 when a reduced distance came within 2^-40 r^2 of r^2 or a squared step within 2^-40 stop^2 of stop^2: only such a seed
+ * may differ from scikit-learn, and the host redoes it). */
+int tgn_meanshift(int n, int n_nodes, const double *Xt, const long long *idx, const int *nodes, const double *bounds, double bandwidth,
+                  double stop_thresh, int max_iter, double *means, int *info, void *stream);
+
 /* Exact float64 kNN with a fused label vote: the answer of sklearn KDTree(xyz).query(queries, k) -- boundary detection of
  * InferencePipeLine.get_boundary_sampled_feats (inference_pipeline_tgn.py:289-330).  xyz (n,3) and queries (m,3) float64
  * DEVICE; 1 <= k <= 64, k <= n.  Distances d2 = (dx*dx + dy*dy) + dz*dz in float64 without contraction, neighbours ascending

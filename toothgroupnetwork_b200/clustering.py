@@ -8,8 +8,11 @@ trained network the DBSCAN alone costs 0.9 s per cloud on the host -- an order o
 Here ``dbscan`` is csrc/dbscan.cu (labels and core samples equal to scikit-learn's: same float64 predicate, same cluster
 numbering, same border rule), the noise vote uses the float64 selection kernel of csrc/crop_knn.cu, and
 ``get_clustering_labels`` keeps the reference's steps and return value.  The elongation test is the reference's (PCA
-eigenvalues of the core points); the MeanShift split, taken for at most three clusters and rarely, stays on scikit-learn.
-``accelerate(ops_utils_module)`` swaps the function in an imported reference ``ops_utils``.
+eigenvalues of the core points); the MeanShift split of at most three elongated clusters is ``MeanShift`` below, whose seed
+ascent is csrc/meanshift.cu (scikit-learn's seeds, centres and labels bit for bit).  ``accelerate(ops_utils_module)`` swaps the
+function in an imported reference ``ops_utils``.
+
+``KMeans`` (csrc/kmeans.cu) is ``ops_utils.clustering_points(method="kmeans")``'s k-means++ / Lloyd fit.
 """
 from __future__ import annotations
 
@@ -145,7 +148,6 @@ def get_clustering_labels(moved_points, labels):
             if eg_first[i] / eg_first[3:].mean() > 8:
                 suspicious.append(order[i])
     for idx, which in enumerate(suspicious):
-        from sklearn.cluster import MeanShift                      # host-side, rare: at most three elongated clusters
         # the reference indexes its list of clusters by position and then rewrites the label equal to that position (:128-132)
         members = fg[dbscan_labels == uniq[which], :3].astype(np.float64)
         split = MeanShift(bandwidth=0.07).fit(members)
@@ -305,3 +307,152 @@ def accelerate_kmeans(module) -> None:
     """Point a module's ``KMeans`` name (``from sklearn.cluster import KMeans`` in ops_utils.py) at the device implementation."""
     if hasattr(module, "KMeans"):
         module.KMeans = KMeans
+
+
+_MS_LEAF_SIZE = 30          # NearestNeighbors' default leaf_size, the tree MeanShift.fit queries
+
+
+def meanshift_device(Xt: torch.Tensor, idx: torch.Tensor, nodes: torch.Tensor, bounds: torch.Tensor, bandwidth: float,
+                     max_iter: int = 300) -> torch.Tensor:
+    """Every seed's ascent of ``MeanShift(bandwidth, max_iter).fit`` on csrc/meanshift.cu, one warp per seed.  The tree is
+    scikit-learn's ``KDTree(X, leaf_size=30).get_arrays()`` on the device: Xt (n,3) float64 = X[idx_array], idx (n) int64 =
+    idx_array, nodes (n_nodes,3) int32 = idx_start, idx_end, is_leaf, bounds (2,n_nodes,3) float64 = node_bounds.  Returns one
+    uint8 buffer of n * 36 bytes: (n,3) float64 final means, then (n,3) int32 member counts, iterations and flags, by index in X
+    (``meanshift_unpack``)."""
+    L.require_cuda(Xt, idx, nodes, bounds)
+    if Xt.dim() != 2 or Xt.shape[1] != 3 or Xt.dtype != torch.float64:
+        raise L.TgnError(f"meanshift expects (n,3) float64 points, got {tuple(Xt.shape)} {Xt.dtype}")
+    n = Xt.shape[0]
+    Xt, idx, nodes, bounds = Xt.contiguous(), idx.long().contiguous(), nodes.int().contiguous(), bounds.double().contiguous()
+    if idx.numel() != n or nodes.dim() != 2 or nodes.shape[1] != 3 or tuple(bounds.shape) != (2, nodes.shape[0], 3):
+        raise L.TgnError(f"meanshift: inconsistent tree arrays idx {tuple(idx.shape)} nodes {tuple(nodes.shape)} bounds {tuple(bounds.shape)}")
+    out = torch.empty(36 * n, dtype=torch.uint8, device=Xt.device)
+    if n:
+        means, info = out[:24 * n].view(torch.float64), out[24 * n:].view(torch.int32)
+        L.call("tgn_meanshift", n, int(nodes.shape[0]), L.ptr(Xt), L.ptr(idx), L.ptr(nodes), L.ptr(bounds), float(bandwidth),
+               1e-3 * bandwidth, int(max_iter), L.ptr(means), L.ptr(info), L.stream_ptr())
+    return out
+
+
+def meanshift_unpack(buf: np.ndarray):
+    """the host copy of ``meanshift_device``'s buffer -> (means (n,3) float64, counts (n), iterations (n), flags (n) bool)"""
+    n = buf.size // 36
+    means = buf[:24 * n].view(np.float64).reshape(n, 3)
+    info = buf[24 * n:].view(np.int32).reshape(n, 3)
+    return means, info[:, 0].astype(np.int64), info[:, 1].astype(np.int64), info[:, 2].astype(bool)
+
+
+def meanshift_tree(X: np.ndarray):
+    """scikit-learn's ``KDTree(X, leaf_size=30)`` (the tree ``NearestNeighbors(radius=...).fit(X)`` builds for n >= 12) as the
+    kernel's arrays: (Xt, idx_array, nodes (n_nodes,3) int32, node_bounds)."""
+    from sklearn.neighbors import KDTree
+    _, idx, node_data, bounds = KDTree(X, leaf_size=_MS_LEAF_SIZE).get_arrays()
+    nodes = np.stack([node_data["idx_start"], node_data["idx_end"], node_data["is_leaf"]], axis=1).astype(np.int32)
+    return np.ascontiguousarray(X[idx]), np.asarray(idx, np.int64), nodes, np.ascontiguousarray(bounds)
+
+
+def meanshift_postprocess(X: np.ndarray, means: np.ndarray, counts: np.ndarray, iters: np.ndarray, bandwidth: float, n_jobs=None):
+    """``MeanShift.fit`` after the seed ascent, made with scikit-learn's own calls: the intensity dict keyed by the mean tuples,
+    the (intensity, tuple) ranking, the near-duplicate pass and the nearest-centre labels -> (cluster_centers_, labels_, n_iter_)."""
+    from sklearn.neighbors import NearestNeighbors
+    center_intensity = {}
+    for mean, c in zip(map(tuple, means), counts.tolist()):
+        if c:
+            center_intensity[mean] = c
+    n_iter = int(max(iters.tolist()))
+    if not center_intensity:
+        raise ValueError(f"No point was within bandwidth={bandwidth:f} of any seed. Try a different seeding strategy "
+                         f"                             or increase the bandwidth.")
+    ranked = sorted(center_intensity.items(), key=lambda tup: (tup[1], tup[0]), reverse=True)
+    sorted_centers = np.array([tup[0] for tup in ranked])
+    unique = np.ones(len(sorted_centers), dtype=bool)
+    nbrs = NearestNeighbors(radius=bandwidth, n_jobs=n_jobs).fit(sorted_centers)
+    for i, center in enumerate(sorted_centers):
+        if unique[i]:
+            unique[nbrs.radius_neighbors([center], return_distance=False)[0]] = 0
+            unique[i] = 1
+    cluster_centers = sorted_centers[unique]
+    _, idxs = NearestNeighbors(n_neighbors=1, n_jobs=n_jobs).fit(cluster_centers).kneighbors(X)
+    return cluster_centers, idxs.flatten(), n_iter
+
+
+def meanshift_seed_host(X: np.ndarray, seed: np.ndarray, nbrs, bandwidth: float, max_iter: int):
+    """one seed's ascent with scikit-learn's public calls (``radius_neighbors``, ``np.mean``, ``np.linalg.norm``), for the seeds
+    the kernel flags -> (mean, count, iterations)"""
+    stop_thresh = 1e-3 * bandwidth
+    it = 0
+    mean = seed
+    while True:
+        members = nbrs.radius_neighbors([mean], bandwidth, return_distance=False)[0]
+        within = X[members]
+        if len(within) == 0:
+            break
+        old = mean
+        mean = np.mean(within, axis=0)
+        if np.linalg.norm(mean - old) <= stop_thresh or it == max_iter:
+            break
+        it += 1
+    return mean, len(within), it
+
+
+class MeanShift:
+    """The slice of ``sklearn.cluster.MeanShift`` the reference uses -- ``MeanShift(bandwidth=0.07).fit(points)`` then
+    ``.labels_`` (ops_utils.py:130 in ``get_clustering_labels``), plus ``.cluster_centers_`` / ``.n_iter_`` -- with the seed
+    ascent on csrc/meanshift.cu, on float64 (n, 3) points.
+
+    The host builds scikit-learn's own KD tree (milliseconds) and hands the kernel its arrays; every seed climbs on the device
+    with scikit-learn's float64 rounding.  Seeds the kernel flags (a distance or a step within 2^-40 relative of the radius or
+    the stop threshold, where scikit-learn's node bounds or another BLAS order could decide otherwise) are redone with
+    scikit-learn's public calls and counted in ``host_seeds``.  The post-processing is scikit-learn's, so cluster_centers_,
+    labels_ and n_iter_ are its own.  Inputs of at most 11 points, which scikit-learn searches by brute force, go to scikit-learn
+    whole (``host_fits``)."""
+
+    host_seeds = 0
+    host_fits = 0
+
+    def __init__(self, bandwidth=None, *, seeds=None, bin_seeding=False, min_bin_freq=1, cluster_all=True, n_jobs=None,
+                 max_iter=300):
+        if bandwidth is None or seeds is not None or bin_seeding or min_bin_freq != 1 or cluster_all is not True:
+            raise L.TgnError(f"MeanShift: only an explicit bandwidth with seeds=None, bin_seeding=False, min_bin_freq=1, "
+                             f"cluster_all=True is implemented (got bandwidth={bandwidth!r}, seeds={'given' if seeds is not None else None}, "
+                             f"bin_seeding={bin_seeding!r}, min_bin_freq={min_bin_freq!r}, cluster_all={cluster_all!r})")
+        if not (isinstance(bandwidth, (int, float, np.integer, np.floating)) and np.isfinite(bandwidth) and bandwidth > 0):
+            raise L.TgnError(f"MeanShift: bandwidth must be a positive finite number, got {bandwidth!r}")
+        if not (isinstance(max_iter, (int, np.integer)) and 0 <= max_iter < 2 ** 31):
+            raise L.TgnError(f"MeanShift: max_iter must be a non-negative int, got {max_iter!r}")
+        self.bandwidth, self.seeds, self.bin_seeding, self.min_bin_freq = bandwidth, seeds, bin_seeding, min_bin_freq
+        self.cluster_all, self.n_jobs, self.max_iter = cluster_all, n_jobs, int(max_iter)
+
+    def fit(self, X, y=None):
+        X = X.detach().cpu().numpy() if isinstance(X, torch.Tensor) else np.asarray(X)
+        if X.dtype != np.float64 or X.ndim != 2 or X.shape[1] != 3:
+            raise L.TgnError(f"MeanShift: expected (n, 3) float64 points, got {X.shape} {X.dtype}")
+        from sklearn.utils import check_array
+        X = check_array(X, dtype=np.float64, order="C")              # scikit-learn's ValueError for NaN, inf and n = 0
+        n, r = X.shape[0], float(self.bandwidth)
+        if n < 12:                                                    # NearestNeighbors picks brute force below 12 points
+            from sklearn.cluster import MeanShift as SkMeanShift
+            type(self).host_fits += 1
+            ref = SkMeanShift(bandwidth=self.bandwidth, n_jobs=self.n_jobs, max_iter=self.max_iter).fit(X)
+            self.cluster_centers_, self.labels_, self.n_iter_ = ref.cluster_centers_, ref.labels_, ref.n_iter_
+            self.n_features_in_ = 3
+            return self
+        if not torch.cuda.is_available():
+            raise L.TgnError("MeanShift needs a CUDA device (there is no CPU path)")
+        Xt, idx, nodes, bounds = meanshift_tree(X)
+        dev = [torch.from_numpy(a).cuda() for a in (Xt, idx, nodes, bounds)]
+        means, counts, iters, flags = meanshift_unpack(meanshift_device(*dev, r, self.max_iter).cpu().numpy())
+        flagged = np.flatnonzero(flags)
+        if flagged.size:
+            from sklearn.neighbors import NearestNeighbors
+            type(self).host_seeds += int(flagged.size)
+            nbrs = NearestNeighbors(radius=r, n_jobs=1).fit(X)
+            means = means.copy()
+            for i in flagged.tolist():
+                means[i], counts[i], iters[i] = meanshift_seed_host(X, X[i], nbrs, r, self.max_iter)
+        self.cluster_centers_, self.labels_, self.n_iter_ = meanshift_postprocess(X, means, counts, iters, r, self.n_jobs)
+        self.n_features_in_ = 3
+        return self
+
+    def fit_predict(self, X, y=None):
+        return self.fit(X).labels_
