@@ -349,6 +349,8 @@ typedef struct {
  *              -> Linear(c/8, c/8) [b_w, b_b]
  *   bn_mode[i]: 1 = batch statistics (stats_* = zeroed fp64 {sum[ch], sumsq[ch]} scratch, filled by the passes), 2 = running
  *   statistics; update_running != 0 applies torch's momentum update to the *_rmean / *_rvar of the BatchNorms in mode 1.
+ *   The passes ADD into stats_*: the caller zeroes them before every launch.
+ *   idx entries must lie in [0, n); they are not checked.
  * c in {32, 64, 128, 256, 512}, K <= 64. */
 typedef struct {
     int n, c, K;

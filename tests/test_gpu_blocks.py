@@ -94,7 +94,15 @@ def test_fused_layer_offset_channels_against_oracle_float64(c, K, n, schedule):
     _layer_against_oracle(c, K, n, True, offset=100.0)
 
 
-def _layer_against_oracle(c, K, n, train_bn, offset):
+@pytest.mark.parametrize("c,K,per_crop", [(512, 24, 12), (256, 24, 48)])
+@pytest.mark.parametrize("train_bn", [True, False])
+def test_fused_layer_16_crops_against_oracle_float64(c, K, per_crop, train_bn, schedule):
+    """the second network's deepest levels: 16 crops packed into one batch (o has 16 offsets); at 12 points per crop every
+    neighbourhood is padded with the crop's first point, as the reference's knnquery pads"""
+    _layer_against_oracle(c, K, 16 * per_crop, train_bn, offset=0.0, crops=16)
+
+
+def _layer_against_oracle(c, K, n, train_bn, offset, crops=1):
     torch.manual_seed(c)
     layer = Layer(c, K).train(train_bn)
     g = torch.Generator().manual_seed(1)
@@ -108,9 +116,9 @@ def _layer_against_oracle(c, K, n, train_bn, offset):
     with torch.no_grad():
         layer.linear_k.bias[0::4] += offset
     state = {k: v.clone() for k, v in layer.state_dict().items()}
-    p = clouds.dental_arch(n, 4)[0].contiguous()
+    p = torch.cat([clouds.dental_arch(n // crops, 4 + k)[0] for k in range(crops)]).contiguous()
     x = torch.randn(n, c, generator=g)
-    o = torch.tensor([n], dtype=torch.int32)
+    o = torch.arange(1, crops + 1, dtype=torch.int32) * (n // crops)
     truth = O.point_transformer_layer(p, x, o, state, K, 8, train_bn, dtype=torch.float64)
     fp32 = O.point_transformer_layer(p, x, o, state, K, 8, train_bn, dtype=torch.float32)
     layer.cuda()

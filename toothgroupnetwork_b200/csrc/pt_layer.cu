@@ -215,6 +215,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
         if (PASS == 3 && !CTAQ) {
 #pragma unroll
             for (int q = 0; q < CPL; ++q) L.out[static_cast<size_t>(i) * C + 32 * q + lane] = out[q];
+            __syncwarp();                                          // the next query's logits overwrite the weights read above
         }
         if (PASS == 3 && CTAQ) {
 #pragma unroll
