@@ -381,6 +381,12 @@ int tgn_pw_fill(float *ptr, long long n, float value, void *stream);
 /* out[b*cout + c] = sum_k w[c*w_row_stride + k] * g[b*g_batch_stride + k], k < cin, accumulated in fp64 and rounded once */
 int tgn_pw_cloud_bias(int B, int cout, int cin, const float *w, long long w_row_stride, const float *g, long long g_batch_stride,
                       float *out, void *stream);
+/* PointNet's per-cloud transforms (pw_transform.cu): out[b, j, n] = sum_{i < ct} x[b, i, n] * t[b*t_batch_stride + i*ct + j] for
+ * j < ct (fp32 FFMA from +0 in increasing i), and out[b, ct + c, n] = x[b, ct + c, n] bit for bit for c < cpass.  x and out are
+ * addressed through (batch, channel, point) element strides and must not overlap.  1 <= ct <= 128. */
+int tgn_pw_cloud_transform(int B, int N, int ct, int cpass, const float *x, long long xs_b, long long xs_c, long long xs_n,
+                           const float *t, long long t_batch_stride, float *out, long long os_b, long long os_c, long long os_n,
+                           void *stream);
 
 #ifdef __cplusplus
 }

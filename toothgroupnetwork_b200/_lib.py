@@ -57,6 +57,8 @@ _SIGS = {
     "tgn_pw_apply": [_vp, _vp],
     "tgn_pw_fill": [_vp, ctypes.c_longlong, _f, _vp],
     "tgn_pw_cloud_bias": [_i, _i, _i, _vp, ctypes.c_longlong, _vp, ctypes.c_longlong, _vp, _vp],
+    "tgn_pw_cloud_transform": [_i, _i, _i, _i, _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, ctypes.c_longlong,
+                               _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp],
     "tgn_kmeans": [_i, ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_meanshift": [_i, _i, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _i, _vp, _vp, _vp],
 }

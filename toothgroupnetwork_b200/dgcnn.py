@@ -191,24 +191,13 @@ def fusable(module, x_in) -> bool:
     return not _needs_grad(module, x)
 
 
-class _ColumnSlice:
-    """conv's weight from input channel ``lo`` on, for the packed-weight cache of ``_PwChain`` (keyed by this object)"""
-
-    def __init__(self, conv, lo: int):
-        self.conv, self.lo, self.bias = conv, lo, None
-
-    @property
-    def weight(self) -> torch.Tensor:
-        return self.conv.weight[:, self.lo:]
-
-
 _state = weakref.WeakKeyDictionary()           # module -> (packed-weight cache, conv7's x1|x2|x3 columns); entries go with the module
 
 
 def _chain(module):
     st = _state.get(module)
     if st is None or st[1].conv is not module.conv7[0]:
-        st = _state[module] = (pn2._PwChain(), _ColumnSlice(module.conv7[0], module.conv6[0].out_channels))
+        st = _state[module] = (pn2._PwChain(), pn2._ColumnSlice(module.conv7[0], module.conv6[0].out_channels))
     return st
 
 

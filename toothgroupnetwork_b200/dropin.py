@@ -136,6 +136,17 @@ def accelerate_dgcnn_forward(module=None) -> None:
     dgcnn.accelerate_forward(module)
 
 
+def accelerate_pointnet_forward(module=None) -> None:
+    """Optional: run the no-grad forward of the PointNet model (``get_model.forward``, models/modules/pointnet.py:23-35) on the
+    tensor-core layer chain of ``toothgroupnetwork_b200.pointnet``: both learned transforms, BatchNorm and the max over the points
+    without the (B, 2176, N) concatenation.  ``PointFirstModule`` calls ``get_model``, so the sem pipeline uses it too.  Under
+    autograd the reference's own forward runs.  Imports ``models.modules.pointnet`` from ``sys.path`` when no module is passed."""
+    from . import pointnet
+    if module is None:
+        module = importlib.import_module("models.modules.pointnet")
+    pointnet.accelerate_forward(module)
+
+
 def uninstall() -> None:
     for alias in _TARGETS:
         sys.modules.pop(alias, None)

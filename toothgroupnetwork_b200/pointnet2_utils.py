@@ -473,11 +473,12 @@ class _PwChain:
         desc.in_update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
 
     def run(self, convs, bns, first: "L.PwLayer", rows: int, out: torch.Tensor, out_c_offset: int, rows_per_batch_out: int,
-            group: int = 0, slopes: Optional[Sequence[float]] = None) -> None:
+            group: int = 0, slopes: Optional[Sequence[float]] = None, relu: bool = True) -> None:
         """``first`` describes the operand source of layer 0 (mode / segments / gather fields filled by the
         caller).  group > 0: the last layer reduces max/min over ``group`` consecutive rows (set abstraction)
         and ``out`` is (B, C_total, rows/group/B...); group == 0: ``out`` receives every row (feature propagation).
-        ``slopes``: LeakyReLU(slopes[l]) follows BatchNorm l instead of ReLU (DGCNN); None leaves every ReLU launch as it was."""
+        ``slopes``: LeakyReLU(slopes[l]) follows BatchNorm l instead of ReLU (DGCNN); None leaves every ReLU launch as it was.
+        ``relu=False``: the last BatchNorm is followed by no activation (PointNet's encoder conv3); ``slopes`` takes precedence."""
         dev = out.device
         n = len(convs)
         couts = [c.weight.shape[0] for c in convs]
@@ -529,7 +530,7 @@ class _PwChain:
             a.rows, a.src, a.ymin = rows // group, L.ptr(keep[-2]), L.ptr(keep[-1])
         else:
             a.rows, a.src, a.ymin = rows, L.ptr(prev_y), None
-        a.rows_per_batch, a.channels, a.out_channels, a.out_c_offset, a.relu = rows_per_batch_out, couts[-1], out.shape[1], out_c_offset, 1
+        a.rows_per_batch, a.channels, a.out_channels, a.out_c_offset, a.relu = rows_per_batch_out, couts[-1], out.shape[1], out_c_offset, int(relu)
         a.out = L.ptr(out)
         a.affine, a.stats, a.stat_rows = mode, L.ptr(stats[-1]), rows
         a.gamma, a.beta = L.ptr(bn.weight), L.ptr(bn.bias)
@@ -542,6 +543,18 @@ class _PwChain:
         for b in bns:
             if b.training and b.num_batches_tracked is not None:
                 b.num_batches_tracked.add_(1)
+
+
+class _ColumnSlice:
+    """conv's weight from input channel ``lo`` on, with conv's bias, for the packed-weight cache of ``_PwChain`` (keyed by this
+    object): a layer whose leading input columns are constant over each cloud and are added as a per-cloud bias instead"""
+
+    def __init__(self, conv, lo: int):
+        self.conv, self.lo, self.bias = conv, lo, conv.bias
+
+    @property
+    def weight(self) -> torch.Tensor:
+        return self.conv.weight[:, self.lo:]
 
 
 def _pw_set_abstraction(chain: _PwChain, convs, bns, xyz_t, feats_t, new_xyz_t, gidx, xyz_first: bool, out, c_offset: int) -> None:
