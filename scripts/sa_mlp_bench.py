@@ -5,7 +5,7 @@ on bench.py's own clouds and module.
 
 Each engine is warmed up, then timed with CUDA events over --windows windows of --launches back-to-back launches;
 the median window is reported as ms per launch, with useful TFLOP/s (2 * rows * sum C_l * C_l+1), issued TF32
-TFLOP/s (the tensor engines' padded 3xTF32 MMAs) and that rate as a fraction of the H100 SXM data-sheet dense TF32
+TFLOP/s (the 3xTF32 engine's padded MMAs) and that rate as a fraction of the H100 SXM data-sheet dense TF32
 peak (495 TFLOP/s at 700 W).  The card's name, power limit and max SM clock are read in the same run.
 
     python scripts/sa_mlp_bench.py [--clouds B] [--windows 7] [--launches 20]
@@ -39,14 +39,15 @@ def card():
 
 
 def issued_tf32_macs_per_row(channels):
-    """MACs the tensor engine issues per grouped row, once (3xTF32 issues three times this): layer 0 at K = C_0
-    rounded up to 8, the inner layers at the narrowest of 16/32/48/64 holding every hidden width, the last layer
-    in 64-channel slices at K = the previous width rounded up to 16."""
+    """TF32 MACs the tensor engine issues per grouped row, all three 3xTF32 terms included.  Every layer runs transposed
+    (weights on M, the tile's rows on N).  The inner layers run on 64 weight rows at K = C_0 rounded up to 8, then the
+    previous width rounded up to 16; at inner widths up to 32 the rows pack W_hi and W_lo of a channel (two MMAs per K-step),
+    wider ones hold one channel per row (three).  The last layer runs in 64-channel slices, three MMAs per K-step."""
     L = len(channels) - 1
     np_ = max([16] + [(c + 15) // 16 * 16 for c in channels[1:L]])
     kpad = [(channels[0] + 7) // 8 * 8] + [(c + 15) // 16 * 16 for c in channels[1:L]]
-    inner = sum(k * np_ for k in kpad[:L - 1])
-    return inner + kpad[L - 1] * 64 * ((channels[L] + 63) // 64)
+    inner = sum(k * 64 * (2 if np_ <= 32 else 3) for k in kpad[:L - 1])
+    return inner + kpad[L - 1] * 64 * 3 * ((channels[L] + 63) // 64)
 
 
 def time_engine(fn, windows, launches):
@@ -90,7 +91,7 @@ def main():
     channels = [9] + list(bench.MLP)
     rows = B * S * K
     useful = 2.0 * rows * sum(a * b for a, b in zip(channels[:-1], channels[1:]))
-    issued = 2.0 * 3 * rows * issued_tf32_macs_per_row(channels)
+    issued = 2.0 * rows * issued_tf32_macs_per_row(channels)
     outs, result = {}, {"card": card(), "shape": {"B": B, "S": S, "K": K, "channels": channels}, "engines": {}}
     for name, engine in (("TC", pn2.ENGINE_TC), ("TC_HALF", pn2.ENGINE_TC_HALF), ("FP32", pn2.ENGINE_FP32)):
         out = torch.empty((B, channels[-1], S), device=dev)

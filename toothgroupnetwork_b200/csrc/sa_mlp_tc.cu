@@ -1,31 +1,34 @@
 // sa_mlp_tc.cu -- warpgroup-MMA (wgmma) tensor-core engine of the fused set-abstraction body.
 //
-// Same contract as the fp32 engine in sa_mlp.cu, but the per-layer contraction
-//      D[128 rows, N] = A[128 rows, K] * W[N, K]^T
-// runs on the tensor cores with the accumulator in registers:
+// Same contract as the fp32 engine in sa_mlp.cu, but every layer's contraction runs on the tensor cores TRANSPOSED,
+//      D^T[channel, row] = W[channel, K] * X[row, K]^T,
+// with the weights as the A operand (channels on M), the activation tile as the B operand (N = the 128 rows of a
+// tile) and the accumulator in registers: one m64n128k8 wgmma does the work of four m64n32k8 ones of the row-major
+// form, so a layer is a few wide MMAs instead of many narrow ones, and the fixed issue and completion latency of
+// each MMA is spread over 4x the work.
 //   * a CTA is up to 4 independent TILE GROUPS of 128 threads (one warpgroup each); a group owns one 128-row tile
 //     (128/K neighbourhoods) at a time.  Thread r of the group gathers row r's [xyz_rel | feats] row into the
-//     first layer's operand (the row of the NEXT tile is loaded into registers while this one computes); every
-//     layer then runs as two 64-row wgmma slices, and each slice's epilogue adds the bias, applies ReLU and writes
-//     the next layer's operand from its accumulator fragments -- the grouped tensor and the inter-layer
-//     activations never leave the SM.  The groups share the weights but nothing else (own operand buffers, named
-//     barriers instead of __syncthreads), so while one group waits for its gather or its MMAs the others fill the
-//     issue slots and the tensor pipe;
-//   * inside a group the slices are software-pipelined as one chain (0,0) (0,1) (1,0) (1,1) ...: each slice's
-//     epilogue runs while the next slice's MMAs are in flight (slice h of layer l+1 only needs slice h of layer l,
-//     so it is issued as soon as that epilogue is stored).  Every wgmma sits in control flow that is uniform over
-//     the warpgroup (the group index comes out of a shuffle, loop bounds out of the kernel parameters); partial
-//     tiles run both slices on zero rows and drop them at the store;
-//   * the inner (hidden) layers all run at one padded width NP (16/32/48/64, a template parameter) with
-//     zero-padded weights and biases, so the accumulators are fixed-size arrays and the kernel does not spill;
-//   * operands live in shared memory in the canonical K-major, no-swizzle layout (8x16-byte core matrices;
-//     element (r,k) at (k/4)*LBO + r*16 + (k%4)*4 with SBO = 128 B);
+//     first layer's operand (the row of the NEXT tile is loaded into registers while this one computes); each
+//     inner layer's epilogue adds the bias, applies ReLU and writes the next layer's operand from its
+//     channel-major accumulator fragments -- the grouped tensor and the inter-layer activations never leave the
+//     SM.  The groups share the weights but nothing else (own operand buffers, named barriers instead of
+//     __syncthreads), so while one group waits for its gather, its MMAs or its epilogue the others fill the issue
+//     slots and the tensor pipe.  Every wgmma sits in control flow that is uniform over the warpgroup (the group
+//     index comes out of a shuffle, loop bounds out of the kernel parameters); partial tiles run on zero rows and
+//     drop them at the store;
 //   * fp32 fidelity: inputs are split a = a_hi + a_lo with a_hi the tf32 truncation, and each K-step issues
-//     three tf32 MMAs (hi*hi + lo*hi + hi*lo) into the same accumulator ("3xTF32"), so the result carries
-//     ~2^-21 relative error instead of tf32's 2^-10 -- the reference's own default for these 1x1 convolutions is
-//     plain TF32 (SURVEY.md 7.1);
-//   * the LAST layer runs transposed, D^T[channel, row] = W[channel, K] * X[row, K]^T: the weights (zero-padded
-//     to 128 channels) are the A operand and the activation tile is the B operand (N = 128 rows), so a thread's
+//     tf32 MMAs for hi*hi + lo*hi + hi*lo ("3xTF32"), so the result carries ~2^-21 relative error instead of
+//     tf32's 2^-10 -- the reference's own default for these 1x1 convolutions is plain TF32 (SURVEY.md 7.1);
+//   * the inner (hidden) layers all run at one padded width NP (16/32/48/64, a template parameter) with
+//     zero-padded weights and biases, on M = 64 weight rows.  Up to 32 channels the rows are PACKED: rows
+//     16w..16w+7 hold W_hi of channels 8w..8w+7 and rows 16w+8..16w+15 their W_lo, so one MMA against X_hi yields
+//     hi*hi and lo*hi of a channel in the same thread, and a second against X_lo with the W_lo rows zero adds
+//     hi*lo: two m64n128k8 per K-step instead of three on a half-empty M.  Wider layers run one channel per row,
+//     three MMAs per K-step;
+//   * operands live in shared memory in the canonical K-major, no-swizzle layout (8x16-byte core matrices;
+//     element (r,k) at (k/4)*LBO + r*16 + (k%4)*4 with SBO = 128 B).  The activation tile's LBO is 128*16 + 16
+//     bytes: an epilogue's 4-byte stores of one warp (8 channels x 4 rows) then fall in 32 distinct banks;
+//   * the LAST layer's weights are zero-padded to 64 or 128 channels and run 64 channels at a time, so a thread's
 //     accumulator fragment holds two channels across all rows of the tile; the max over the K rows of a
 //     neighbourhood is a chain of max inside the thread plus two shuffles across its quad.
 // Weights are split and laid out once per CTA; CTAs are persistent over tiles.
@@ -45,65 +48,94 @@ constexpr int kRows = 128;                            // rows of a tile = thread
 constexpr int kMaxGroups = 4;                         // tile groups per CTA: 4 (one CTA owns the SM) or 2 (two CTAs per SM, or one
                                                       // beside another kernel's CTAs: 32K registers each)
 constexpr int kInCols = 16;                           // the gathered input row, zero-padded: 3 + D <= 16
-constexpr uint32_t kChunkStrideA = kRows * 16;        // LBO of the A operand: one 16-byte K-chunk of all rows
+constexpr int kInnerM = 64;                           // weight rows (M) of an inner layer's MMA
+constexpr uint32_t kActChunk = kRows * 16 + 16;       // LBO of the activation tile: one 16-byte K-chunk of all rows + 16
+                                                      // bytes, so that the epilogue's stores do not collide in banks
 
 struct TcLayout {
     int kpad[kSaMaxLayers];          // K of layer l: 3 + D rounded up to 8, then the previous layer's width rounded up to 16
-    int np;                          // N of every inner layer (the kernel's template width)
-    uint32_t w_hi[kSaMaxLayers], w_lo[kSaMaxLayers];   // byte offsets in dynamic smem
+    int np;                          // padded width of every inner layer (the kernel's template width)
+    int last_rows;                   // weight rows of the last layer: its width rounded up to 64
+    uint32_t w_a[kSaMaxLayers], w_b[kSaMaxLayers];     // byte offsets in dynamic smem of layer l's two A operands
     uint32_t bias;                   // inner layers' biases, np floats each, zero-padded
-    uint32_t a_hi[kMaxGroups], a_lo[kMaxGroups];   // per group activation operands (A of the inner layers, B of the last)
+    uint32_t a_hi[kMaxGroups], a_lo[kMaxGroups];   // per group activation tile (B operand of every layer), hi / lo
     int groups;                      // tile groups per CTA
     uint32_t total;
     int tiles_per_cloud, gpt;
     uint32_t tpc_magic;              // floor(2^32 / tiles_per_cloud): t / tiles_per_cloud by IMAD.HI + one fix-up
 };
 
-// Issue the 3xTF32 MMAs of one inner layer on one 64-row slice (rows 64h..64h+63) of a group's tile as one wgmma group:
-// acc = X[rows, 0..kp) * W[NP, 0..kp)^T.  The first MMA writes acc without reading it, so acc is not cleared: an
-// instruction that wrote it while the other slice's MMAs are in flight would make the compiler serialise them.
+// Inner layers of width <= 32 pack W_hi and W_lo of a channel into one 64-row A operand (file comment).
 template <int NP>
-__device__ __forceinline__ void issue_slice(float (&acc)[NP / 2], int h, int kp, uint32_t a_hi, uint32_t a_lo, uint32_t w_hi,
-                                            uint32_t w_lo)
+constexpr bool kPacked = NP <= 32;
+
+// Issue the 3xTF32 MMAs of one inner layer on a group's whole tile as one wgmma group: acc = W[64, 0..kp) *
+// X[128 rows, 0..kp)^T.  The first MMA writes acc without reading it, so acc is not cleared.
+template <int NP>
+__device__ __forceinline__ void issue_inner(float (&acc)[64], int kp, uint32_t x_hi, uint32_t x_lo, uint32_t w_a, uint32_t w_b)
 {
-    constexpr uint32_t lbo_w = NP * 16;
-    uint64_t d_xhi = make_smem_desc(a_hi + h * 64 * 16, kChunkStrideA), d_xlo = make_smem_desc(a_lo + h * 64 * 16, kChunkStrideA);
-    uint64_t d_whi = make_smem_desc(w_hi, lbo_w), d_wlo = make_smem_desc(w_lo, lbo_w);
+    constexpr uint32_t lbo_w = kInnerM * 16;
+    uint64_t d_xhi = make_smem_desc(x_hi, kActChunk), d_xlo = make_smem_desc(x_lo, kActChunk);
+    uint64_t d_wa = make_smem_desc(w_a, lbo_w), d_wb = make_smem_desc(w_b, lbo_w);
+    auto rest = [&] {
+        if (kPacked<NP>) {
+            wgmma_tf32<128>(acc, d_wb, d_xlo, true);            // [W_hi | 0] * X_lo
+        } else {
+            wgmma_tf32<128>(acc, d_wa, d_xlo, true);            // W_hi * X_lo
+            wgmma_tf32<128>(acc, d_wb, d_xhi, true);            // W_lo * X_hi
+        }
+    };
     wgmma_fence();
-    wgmma_tf32_zero<NP>(acc, d_xhi, d_whi);
-    wgmma_tf32<NP>(acc, d_xlo, d_whi, true);
-    wgmma_tf32<NP>(acc, d_xhi, d_wlo, true);
+    wgmma_tf32_zero<128>(acc, d_wa, d_xhi);
+    rest();
     for (int ks = 1; ks < kp / 8; ++ks) {
-        d_xhi += desc_step(2 * kChunkStrideA); d_xlo += desc_step(2 * kChunkStrideA);
-        d_whi += desc_step(2 * lbo_w); d_wlo += desc_step(2 * lbo_w);
-        wgmma_tf32<NP>(acc, d_xhi, d_whi, true);
-        wgmma_tf32<NP>(acc, d_xlo, d_whi, true);
-        wgmma_tf32<NP>(acc, d_xhi, d_wlo, true);
+        d_xhi += desc_step(2 * kActChunk); d_xlo += desc_step(2 * kActChunk);
+        d_wa += desc_step(2 * lbo_w); d_wb += desc_step(2 * lbo_w);
+        wgmma_tf32<128>(acc, d_wa, d_xhi, true);
+        rest();
     }
     wgmma_commit();
 }
 
-// Epilogue of one finished slice: + bias, ReLU, tf32 hi/lo split and 8-byte stores of the fragment pairs into the next
-// layer's K-major operand (the same buffers: the slice only overwrites its own rows, which no other slice reads).
+// Epilogue of a finished inner layer: + bias, ReLU, tf32 hi/lo split and 4-byte stores of the thread's channels
+// across the tile's rows into the next layer's K-major operand (the same buffers, rewritten after every warp's MMAs
+// have read them).  Channels from NP on are never read, so the warps that hold only those store nothing.
 template <int NP>
-__device__ __forceinline__ void store_slice(const float (&acc)[NP / 2], int h, uint32_t a_hi, uint32_t a_lo, const float* bias)
+__device__ __forceinline__ void store_inner(const float (&acc)[64], uint32_t x_hi, uint32_t x_lo, const float* bias)
 {
     const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
-    const int row = h * 64 + w * 16 + (lane >> 2);
+    const int r0 = 2 * (lane & 3);                 // the thread's rows: 8i + r0 + e
+    auto put = [&](float v, uint32_t o) {
+        uint32_t hi, lo;
+        split_tf32(fmaxf(v, 0.f), hi, lo);
+        st_shared_b32(x_hi + o, hi);
+        st_shared_b32(x_lo + o, lo);
+    };
+    if (kPacked<NP>) {
+        // rows 16w + lane/4 (hi*hi + hi*lo) and 16w + 8 + lane/4 (lo*hi) of D^T are the parts of channel 8w + lane/4
+        if (8 * w >= NP) return;
+        const int c = 8 * w + (lane >> 2);
+        const float b = bias[c];
+        const uint32_t off = static_cast<uint32_t>(c >> 2) * kActChunk + (c & 3) * 4 + r0 * 16;
 #pragma unroll
-    for (int i = 0; i < NP / 8; ++i) {
-        const int c = 8 * i + 2 * (lane & 3);
-        const float b0 = bias[c], b1 = bias[c + 1];
-        const uint32_t off = static_cast<uint32_t>(c >> 2) * kChunkStrideA + (c & 3) * 4;
+        for (int i = 0; i < 16; ++i)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            uint32_t hi0, lo0, hi1, lo1;
-            split_tf32(fmaxf(acc[4 * i + 2 * e] + b0, 0.f), hi0, lo0);
-            split_tf32(fmaxf(acc[4 * i + 2 * e + 1] + b1, 0.f), hi1, lo1);
-            const uint32_t o = off + (row + 8 * e) * 16;
-            st_shared_v2(a_hi + o, hi0, hi1);
-            st_shared_v2(a_lo + o, lo0, lo1);
-        }
+            for (int e = 0; e < 2; ++e) put((acc[4 * i + e] + acc[4 * i + 2 + e]) + b, off + (8 * i + e) * 16);
+    } else {
+        // rows 16w + lane/4 and 16w + 8 + lane/4 of D^T are channels c and c + 8
+        if (16 * w >= NP) return;
+        const bool second = 16 * w + 8 < NP;
+        const int c = 16 * w + (lane >> 2);
+        const float b0 = bias[c], b1 = second ? bias[c + 8] : 0.f;
+        const uint32_t off0 = static_cast<uint32_t>(c >> 2) * kActChunk + (c & 3) * 4 + r0 * 16;
+        const uint32_t off1 = off0 + 2 * kActChunk;
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                put(acc[4 * i + e] + b0, off0 + (8 * i + e) * 16);
+                if (second) put(acc[4 * i + 2 + e] + b1, off1 + (8 * i + e) * 16);
+            }
     }
 }
 
@@ -118,22 +150,25 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
     // tile group, read through a shuffle so that the compiler sees it (and everything derived from it: the tile
     // loop, every wgmma) as warp-uniform -- otherwise it serialises the asynchronous MMAs
     const int g = __shfl_sync(0xffffffffu, tid / kRows, 0);
-    const int r = tid - g * kRows;             // row inside the tile (inner layers) / output channel (last layer)
-    // ---- weights: split into tf32 hi/lo, canonical K-major layout.  Inner layers: B operand
-    //      [NP x kpad] (LBO = NP*16); last layer: A operand [128 x kpad] (LBO = 128*16).  Zero rows
-    //      beyond cout.  SBO = 128 either way.  Biases are added in fp32 by the epilogues.
+    const int r = tid - g * kRows;             // row of the tile this thread gathers
+    // ---- weights: split into tf32 hi/lo, canonical K-major A operands [M x kpad] (LBO = M*16, SBO = 128): M = 64
+    //      for the inner layers (packed or one channel per row, see the file comment), 64 or 128 for the last layer
+    //      (w_a = W_hi, w_b = W_lo).  Zero rows beyond cout.  Biases are added in fp32 by the epilogues.
     float* bias_s = reinterpret_cast<float*>(smem + lay.bias);
     for (int l = 0; l < p.L; ++l) {
         const int cin = p.ch[l], cout = p.ch[l + 1], kp = lay.kpad[l];
-        const int np = l == p.L - 1 ? kRows : NP;
-        for (int e = tid; e < np * kp; e += kThreads) {
-            const int n = e / kp, k = e - n * kp;
+        const bool inner = l < p.L - 1, packed = inner && kPacked<NP>;
+        const int m_rows = inner ? kInnerM : lay.last_rows;
+        for (int e = tid; e < m_rows * kp; e += kThreads) {
+            const int m = e / kp, k = e - m * kp;
+            const int n = packed ? (m >> 4) * 8 + (m & 7) : m;          // channel of weight row m
+            const bool lo_row = packed && (m & 8);
             const float w = (n < cout && k < cin) ? __ldg(p.W[l] + static_cast<size_t>(n) * cin + k) : 0.f;
             uint32_t hi, lo;
             split_tf32(w, hi, lo);
-            const uint32_t off = static_cast<uint32_t>(k >> 2) * (np * 16) + n * 16 + (k & 3) * 4;
-            *reinterpret_cast<uint32_t*>(smem + lay.w_hi[l] + off) = hi;
-            *reinterpret_cast<uint32_t*>(smem + lay.w_lo[l] + off) = lo;
+            const uint32_t off = static_cast<uint32_t>(k >> 2) * (m_rows * 16) + m * 16 + (k & 3) * 4;
+            *reinterpret_cast<uint32_t*>(smem + lay.w_a[l] + off) = lo_row ? lo : hi;
+            *reinterpret_cast<uint32_t*>(smem + lay.w_b[l] + off) = packed ? (lo_row ? 0u : hi) : lo;
         }
         if (l < p.L - 1)
             for (int c = tid; c < NP; c += kThreads) bias_s[l * NP + c] = c < cout ? __ldg(p.bias[l] + c) : 0.f;
@@ -208,7 +243,7 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
             uint32_t hi[4], lo[4];
 #pragma unroll
             for (int i = 0; i < 4; ++i) split_tf32(row[4 * kc + i], hi[i], lo[i]);
-            const uint32_t off = kc * kChunkStrideA + r * 16;
+            const uint32_t off = kc * kActChunk + r * 16;
             st_shared_v4(a_hi + off, hi[0], hi[1], hi[2], hi[3]);
             st_shared_v4(a_lo + off, lo[0], lo[1], lo[2], lo[3]);
         }
@@ -217,48 +252,26 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
         proxy_fence_async();               // this thread's operand stores -> visible to the tensor core
         group_sync(g);
 
-        // ---- inner layers: each slice's epilogue runs under the MMAs of the next slice in the chain
-        //      (l,0) (l,1) (l+1,0) (l+1,1) ...; slice h of layer l+1 only needs slice h of layer l.  Every epilogue
-        //      follows a wait for ALL issued MMAs and the next slice is issued after it: the compiler serialises
-        //      the MMAs when an accumulator is read while a group issued before it is still open, or when the
-        //      open groups differ between paths (hence the last inner layer is peeled).
-        if (n_inner > 0) {
-            float acc0[NP / 2], acc1[NP / 2];
-            auto finish = [&](const float (&acc)[NP / 2], int h, int l) {
-                group_sync(g);             // every warp's MMAs have read the slice's rows before any of them is overwritten
-                store_slice<NP>(acc, h, a_hi, a_lo, bias_s + l * NP);
-                proxy_fence_async();
-                group_sync(g);
-            };
-            issue_slice<NP>(acc0, 0, lay.kpad[0], a_hi, a_lo, sbase + lay.w_hi[0], sbase + lay.w_lo[0]);
-            int l = 0;
-            for (; l < n_inner - 1; ++l) {
-                const uint32_t whi = sbase + lay.w_hi[l], wlo = sbase + lay.w_lo[l];
-                wgmma_wait<0>();
-                fence_regs(acc0);
-                issue_slice<NP>(acc1, 1, lay.kpad[l], a_hi, a_lo, whi, wlo);
-                finish(acc0, 0, l);
-                wgmma_wait<0>();
-                fence_regs(acc1);
-                issue_slice<NP>(acc0, 0, lay.kpad[l + 1], a_hi, a_lo, sbase + lay.w_hi[l + 1], sbase + lay.w_lo[l + 1]);
-                finish(acc1, 1, l);
-            }
+        // ---- inner layers: the whole tile's MMAs as one group, then the epilogue rewrites the operand in place
+        for (int l = 0; l < n_inner; ++l) {
+            float acc[64];
+            issue_inner<NP>(acc, lay.kpad[l], a_hi, a_lo, sbase + lay.w_a[l], sbase + lay.w_b[l]);
             wgmma_wait<0>();
-            fence_regs(acc0);
-            issue_slice<NP>(acc1, 1, lay.kpad[l], a_hi, a_lo, sbase + lay.w_hi[l], sbase + lay.w_lo[l]);
-            finish(acc0, 0, l);
-            wgmma_wait<0>();
-            fence_regs(acc1);
-            finish(acc1, 1, l);
+            fence_regs(acc);
+            group_sync(g);                 // every warp's MMAs have read the tile before any of it is overwritten
+            store_inner<NP>(acc, a_hi, a_lo, bias_s + l * NP);
+            proxy_fence_async();
+            group_sync(g);
         }
 
         // ---- last layer: D^T[channel, row] += W[channel, k] * X[row, k], one 64-channel slice at a time
         const int l = p.L - 1, kp = lay.kpad[l];
         float* ob = p.out + (static_cast<size_t>(b) * p.out_c_total + p.out_c_offset) * p.S;
+        const uint32_t lbo_w = lay.last_rows * 16;
         for (int hc = 0; 64 * hc < cout_last; ++hc) {
-            uint64_t d_whi = make_smem_desc(sbase + lay.w_hi[l] + hc * 64 * 16, kChunkStrideA);
-            uint64_t d_wlo = make_smem_desc(sbase + lay.w_lo[l] + hc * 64 * 16, kChunkStrideA);
-            uint64_t d_xhi = make_smem_desc(a_hi, kChunkStrideA), d_xlo = make_smem_desc(a_lo, kChunkStrideA);
+            uint64_t d_whi = make_smem_desc(sbase + lay.w_a[l] + hc * 64 * 16, lbo_w);
+            uint64_t d_wlo = make_smem_desc(sbase + lay.w_b[l] + hc * 64 * 16, lbo_w);
+            uint64_t d_xhi = make_smem_desc(a_hi, kActChunk), d_xlo = make_smem_desc(a_lo, kActChunk);
             float acc[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -268,8 +281,8 @@ sa_mlp_tc_kernel(const SaParams p, const TcLayout lay)
                 wgmma_tf32<128>(acc, d_whi, d_xhi, ks > 0);
                 wgmma_tf32<128>(acc, d_whi, d_xlo, true);
                 wgmma_tf32<128>(acc, d_wlo, d_xhi, true);
-                d_xhi += desc_step(2 * kChunkStrideA); d_xlo += desc_step(2 * kChunkStrideA);
-                d_whi += desc_step(2 * kChunkStrideA); d_wlo += desc_step(2 * kChunkStrideA);
+                d_xhi += desc_step(2 * kActChunk); d_xlo += desc_step(2 * kActChunk);
+                d_whi += desc_step(2 * lbo_w); d_wlo += desc_step(2 * lbo_w);
             }
             wgmma_commit();
             wgmma_wait<0>();
@@ -295,6 +308,7 @@ bool make_layout(const SaParams& p, TcLayout& lay, int kGroups = kMaxGroups)
     if (p.ch[0] > kInCols) return false;                 // the gathered row is built in 16 registers
     lay.np = inner_width(p);
     if (lay.np == 0) return false;
+    lay.last_rows = (p.ch[p.L] + 63) / 64 * 64;
     int kmax = kInCols;
     uint32_t off = 0;
     auto take = [&off](uint32_t bytes, uint32_t align) {
@@ -308,16 +322,16 @@ bool make_layout(const SaParams& p, TcLayout& lay, int kGroups = kMaxGroups)
         kmax = std::max(kmax, lay.kpad[l]);
     }
     kmax = std::max(kmax, p.L > 1 ? lay.np : 0);       // the inner layers' epilogues write np columns
-    const uint32_t a_bytes = static_cast<uint32_t>(kmax / 4) * kChunkStrideA;
+    const uint32_t a_bytes = static_cast<uint32_t>(kmax / 4) * kActChunk;
     for (int g = 0; g < kGroups; ++g) {
         lay.a_hi[g] = take(a_bytes, 128);
         lay.a_lo[g] = take(a_bytes, 128);
     }
     for (int l = 0; l < p.L; ++l) {
-        const int rows_w = l == p.L - 1 ? kRows : lay.np;      // the last layer's weights are a 128-row A operand
+        const int rows_w = l == p.L - 1 ? lay.last_rows : kInnerM;
         const uint32_t wb = static_cast<uint32_t>(rows_w) * lay.kpad[l] * 4;
-        lay.w_hi[l] = take(wb, 128);
-        lay.w_lo[l] = take(wb, 128);
+        lay.w_a[l] = take(wb, 128);
+        lay.w_b[l] = take(wb, 128);
     }
     lay.bias = take(static_cast<uint32_t>(std::max(p.L - 1, 1) * lay.np) * 4, 16);
     lay.total = off;
@@ -361,7 +375,7 @@ int launch_tc(const SaParams& p, const TcLayout& lay, cudaStream_t st)
 // groups_per_cta: 4 = one CTA owns the SM (all 64K registers); 2 = half-size CTAs (32K registers) that can share an SM with
 // the CTAs of another stream's kernels -- the host pipeline keeps the FPS of the
 // next chunk resident, and a full-size CTA would wait for it to drain.  (Two half CTAs fit one SM only when the operand
-// tiles are small; with the bench shape the weights of the 128-row last layer make it one per SM.)
+// tiles are small: with the bench shape each takes 105 KB of shared memory, so two do.)
 int sa_mlp_tc_launch(SaParams p, cudaStream_t st, int groups_per_cta)
 {
     TcLayout lay{};
