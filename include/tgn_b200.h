@@ -351,7 +351,7 @@ typedef struct {
  *   statistics; update_running != 0 applies torch's momentum update to the *_rmean / *_rvar of the BatchNorms in mode 1.
  *   The passes ADD into stats_*: the caller zeroes them before every launch.
  *   idx entries must lie in [0, n); they are not checked.
- * c in {32, 64, 128, 256, 512}, K <= 64. */
+ * c in {16, 32, 64, 128, 256, 512}, K <= 64; c = 16 runs two queries per warp, one per half-warp. */
 typedef struct {
     int n, c, K;
     const float *p, *xq, *xk, *xv;
@@ -369,7 +369,8 @@ typedef struct {
 } tgn_pt_layer_t;
 int tgn_pt_layer_forward(const tgn_pt_layer_t *layer, void *stream);
 int tgn_pt_layer_struct_size(void);
-/* layers with fewer queries than this run one CTA per query instead of one warp per query (default 1024); returns the old value */
+/* layers with fewer queries than this run one CTA per query instead of one warp per query (default 1024); returns the old value.
+ * c = 16 layers always run two queries per warp: the threshold does not apply to them. */
 int tgn_pt_layer_set_cta_threshold(int n_queries);
 
 size_t tgn_pw_packed_bytes(int cout, int cin);

@@ -2,7 +2,7 @@
 """Model-level parity + timing of the reference's REAL model files on the two operator sets
 (VERDICT r1 item 1; SURVEY.md 8d configs C2-model, C3, C4).
 
-    python scripts/model_parity.py [--out gpurun_out/model_parity.json] [--points 24000] [--cases pp,tseg,tgn]
+    python scripts/model_parity.py [--out PATH.json] [--points 24000] [--cases pp,tseg,tgn,tgni,tgnb]
 
 For each case the reference's unmodified ``models/modules/*.py`` is built twice in this process
 (``oracle/ref_models.World``): once on the reference's own operators (verbatim ``pointops`` kernels
@@ -33,6 +33,10 @@ Cases
         ``seg_module`` on (8, 36, 3072).  The DBSCAN step (``tsegnet.py:57-71``) needs trained offsets
         to find clusters; with random-init weights the 8 crop centres are the GT tooth centroids instead.
   tgn   ``GroupingNetworkModule`` forward + backward, ``train_configs/tgnet_fps.py:27-36`` parameters.
+  tgni  the same module under no_grad (validation form, labels given), train- and eval-mode BN; fused and unfused blocks timed.
+  tgnb  the boundary network (``train_configs/tgnet_bdl.py``: planes [16, 32], stride [1, 1], nsample [36, 24]) under no_grad
+        in the form the tgnet inference pipeline calls it (``test=True``, inference_pipeline_tgn.py:229), train-mode BN; its
+        c = 16 transformer layers run on the fused kernel's half-warp schedule.  Fused and unfused blocks timed.
 
 This is test infrastructure: it imports ``oracle/``.  ``--cpu-dry-run`` exercises the harness on the
 reference world only (oracle FPS/kNN on CPU, small cloud) in a GPU-less container.
@@ -62,6 +66,8 @@ TRUTH_FACTOR = 2.0
 NOISE_FACTOR = 3.0
 TGN_PARAMS = {"input_feat": 6, "stride": [1, 4, 4, 4, 4], "nsample": [36, 24, 24, 24, 24], "blocks": [2, 3, 4, 6, 3],
               "block_num": 5, "planes": [32, 64, 128, 256, 512], "crop_sample_size": 3072}
+TGNB_PARAMS = {"input_feat": 6, "stride": [1, 1], "nsample": [36, 24], "blocks": [2, 3], "block_num": 2, "planes": [16, 32],
+               "crop_sample_size": 3072}
 
 
 def dev(t):
@@ -360,11 +366,13 @@ def case_tgn(worlds, feats, labels, timer):
     return res
 
 
-def case_tgn_infer(worlds, feats, labels, train_bn, timer):
+def case_tgn_infer(worlds, feats, labels, train_bn, timer, params=TGN_PARAMS, test=False):
     """GroupingNetworkModule forward under torch.no_grad() with labels given (the reference's validation step,
     grouping_network_module.py:25-35,46-57: crops around the ground-truth centroids; the label-free inference branch :58-69 clusters
     the predicted offsets instead, which needs trained weights -- tests/test_gpu_clustering.py covers that function): in the b200 world the
-    PointTransformerLayer and TransitionDown forwards run on the fused kernels (toothgroupnetwork_b200.blocks_fused)."""
+    PointTransformerLayer and TransitionDown forwards run on the fused kernels (toothgroupnetwork_b200.blocks_fused).
+    ``params`` is the model_parameter dict (TGN_PARAMS: the first network; TGNB_PARAMS: the boundary network); ``test=True`` is the
+    forward's test flag, as the inference pipeline passes it (the first model then runs without labels; crops still follow them)."""
     outs, coords, times = {}, {}, {}
     state = None
     keys = ("sem_1", "offset_1", "first_features", "sem_2", "cropped_feature_ls")
@@ -372,7 +380,7 @@ def case_tgn_infer(worlds, feats, labels, train_bn, timer):
         with w, torch.no_grad():
             torch.manual_seed(0)
             gm = w.mod("models.modules.grouping_network_module")
-            module = dev(gm.GroupingNetworkModule({"model_parameter": dict(TGN_PARAMS)}))
+            module = dev(gm.GroupingNetworkModule({"model_parameter": dict(params)}))
             if state is None:
                 state = {k: v.clone() for k, v in module.state_dict().items()}
             module.train(train_bn)
@@ -382,7 +390,7 @@ def case_tgn_infer(worlds, feats, labels, train_bn, timer):
             def fwd():
                 module.load_state_dict(state)                      # same running statistics every repetition
                 coords[w.ops].clear()
-                return module([feats, labels])
+                return module([feats, labels], test=test)
 
             o, ms = timer(fwd, warm=1, reps=3)
             outs[w.ops] = {k: o[k] for k in keys if o.get(k) is not None}
@@ -408,7 +416,7 @@ def case_tgn_infer(worlds, feats, labels, train_bn, timer):
                     with float64_point_transformer(w):
                         module.load_state_dict(state)
                         module.double()
-                        o = module([feats.double(), labels])
+                        o = module([feats.double(), labels], test=test)
                         outs["fp64_truth"] = {k: o[k] for k in keys if o.get(k) is not None}
                         outs["fp64_truth"]["nn_crop_indexes"] = torch.from_numpy(np.stack([np.asarray(x) for x in o["nn_crop_indexes"]]).astype(np.int64))
                 except Exception as e:                             # the truth leg is an aid, not the gate
@@ -484,6 +492,8 @@ def main():
     if "tgni" in cases:
         report["tgnet_fps_nograd_trainBN"] = case_tgn_infer(worlds, feats, labels, True, timer)
         report["tgnet_fps_nograd_evalBN"] = case_tgn_infer(worlds, feats, labels, False, timer)
+    if "tgnb" in cases:
+        report["tgnet_bdl_nograd_test_trainBN"] = case_tgn_infer(worlds, feats, labels, True, timer, params=TGNB_PARAMS, test=True)
     os.makedirs(os.path.dirname(args.out), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(report, f, indent=1)

@@ -1,7 +1,12 @@
 """Fused PointTransformerLayer forward (csrc/pt_layer.cu) per level of the tgnet_fps encoder: warp-per-query against CTA-per-query
-schedule, and the reference's unfused torch code on this package's operators, train-mode BatchNorm, no_grad."""
+schedule, and the reference's unfused torch code on this package's operators, train-mode BatchNorm, no_grad.
+
+The boundary network's c = 16 level (tgnet_bdl: 24 000 points, or 16 crops of 3 072) has one schedule (two queries per warp), so its
+rows time the fused layer against the unfused code only: five alternating rounds of each, the median reported."""
 import json
 import os
+import statistics
+import subprocess
 import sys
 
 import torch
@@ -44,9 +49,30 @@ def time_ms(fn, reps=20):
     return e0.elapsed_time(e1) / reps
 
 
+def c16_row(K, n):
+    """fused against unfused at c = 16, alternated within one process so that both see the same clocks and neighbours"""
+    layer = Layer(16, K).cuda().train()
+    p = clouds.dental_arch(n, 1)[0].cuda().contiguous()
+    x = torch.randn(n, 16, device="cuda")
+    o = torch.tensor([n], dtype=torch.int32, device="cuda")
+    fused, ref = [], []
+    with torch.no_grad():
+        for _ in range(5):
+            fused.append(time_ms(lambda: blocks_fused.pt_layer_forward(layer, [p, x, o]), reps=100))
+            ref.append(time_ms(lambda: unfused(layer, p, x, o), reps=20))
+    return {"c": 16, "K": K, "n": n, "default_ms": statistics.median(fused), "unfused_torch_ms": statistics.median(ref),
+            "default_ms_rounds": fused, "unfused_torch_ms_rounds": ref}
+
+
 def main():
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                          capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"device": torch.cuda.get_device_name(0), "name_power_limit_max_sm_clock": card}))
     rows = []
     lib = L.load()
+    for K, n in ((36, 24000), (36, 49152)):
+        rows.append(c16_row(K, n))
+        print(json.dumps(rows[-1]))
     for c, K, n in ((32, 36, 24000), (64, 24, 6000), (128, 24, 1500), (256, 24, 375), (512, 24, 93), (32, 36, 49152), (64, 24, 12288), (128, 24, 3072)):
         layer = Layer(c, K).cuda().train()
         p = clouds.dental_arch(n, 1)[0].cuda().contiguous()

@@ -21,7 +21,7 @@ from . import _lib as L
 from . import pointnet2_utils as pn2
 from . import pointops
 
-_SUPPORTED_C = (32, 64, 128, 256, 512)
+_SUPPORTED_C = (16, 32, 64, 128, 256, 512)
 _enabled = True
 
 

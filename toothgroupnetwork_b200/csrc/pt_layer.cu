@@ -20,7 +20,14 @@
 // CTA, turned into scale / shift in the next pass's prologue.  With running statistics (eval mode) only pass 3 runs.
 // One warp per query; lane l owns channels l, l + 32, ... (CPL = c / 32 of them); the c -> c/8 product is per-lane partial
 // sums + a butterfly, so every lane ends up with all c/8 values; logits of the K neighbours wait in shared memory for the
-// softmax.  fp32 FMA arithmetic throughout.  Shapes: c in {32, 64, 128, 256, 512}, share_planes = 8, K <= 64.
+// softmax.  fp32 FMA arithmetic throughout.  Shapes: c in {16, 32, 64, 128, 256, 512}, share_planes = 8, K <= 64.
+//
+// c = 16 (the boundary network's first level) runs two queries per warp, one per half-warp (W = 16 lanes per query): lane l owns
+// channel l & 15 of query 2 w + (l >> 4), the c -> c/8 butterfly stays inside the half (xor 8, 4, 2, 1), and each half has its
+// own logits.  One warp per query would leave 16 of 32 lanes idle in an fp32-issue-bound kernel.  The grid-stride loop steps over
+// query PAIRS so that both halves run the same trip count: a half without a query (odd n, the end of the stride) computes on a
+// clamped index and keeps nothing, because it still has to take part in every full-mask shuffle and __syncwarp.  The CTA-per-query
+// schedule (tgn_pt_layer_set_cta_threshold) is for wide channels at deep levels and does not apply to c = 16.
 #include <algorithm>
 
 #include "common.cuh"
@@ -65,18 +72,22 @@ __device__ __forceinline__ float bn_relu(float x, const BnAffine& a)
 // CTAQ = true : one CTA per query, its warps take the neighbours round-robin and meet in shared memory for the softmax and the
 //               output sum (deep levels: a few hundred queries of 128-512 channels, where a single warp walking K neighbours
 //               times c/8 x c products is pure latency).
-template <int CPL, int PASS, bool CTAQ>
+// W = 16: two queries per warp, one per half-warp (c = 16 only).
+template <int CPL, int PASS, bool CTAQ, int W = 32>
 __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_layer_t L)
 {
-    constexpr int C = 32 * CPL, CS = 4 * CPL;                  // channels, channels / share_planes (= 8)
+    static_assert(W == 32 || (W == 16 && CPL == 1 && !CTAQ), "half-warp queries: c = 16, warp schedule only");
+    constexpr int C = W * CPL, CS = C / 8;                     // channels, channels / share_planes (= 8)
+    constexpr int QPW = 32 / W;                                // queries per warp
     extern __shared__ __align__(16) unsigned char dyn[];
     BnAffine* ss_a = reinterpret_cast<BnAffine*>(dyn);         // [C]   BatchNorm_a mean / scale / beta
     BnAffine* ss_b = ss_a + C;                                 // [CS]  BatchNorm_b
     BnAffine* ss_p = ss_b + CS;                                // [4]   BatchNorm_p (3 used)
-    float* logits_all = reinterpret_cast<float*>(ss_p + 4);    // [kWarps][K][CS]; CTAQ: [K][CS] then [kWarps][C] output partials
+    float* logits_all = reinterpret_cast<float*>(ss_p + 4);    // [kWarps * QPW][K][CS]; CTAQ: [K][CS] then [kWarps][C] output partials
     __shared__ double red[kWarps][8];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int sl = lane & (W - 1), half = lane / W;            // lane within the query's lanes, the query's slot in the warp
     const double cnt = static_cast<double>(L.n) * L.K;
     if (PASS >= 1) for (int a = tid; a < 3; a += kWarps * 32)
         ss_p[a] = scale_shift(L.bn_mode[0], a, 3, L.stats_p, cnt, L.p_gamma, L.p_beta, L.p_eps, L.p_rmean, L.p_rvar);
@@ -85,7 +96,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
     if (PASS >= 3) for (int m = tid; m < CS; m += kWarps * 32)
         ss_b[m] = scale_shift(L.bn_mode[2], m, CS, L.stats_b, cnt, L.b_gamma, L.b_beta, L.b_eps, L.b_rmean, L.b_rvar);
     __syncthreads();
-    float* logits = CTAQ ? logits_all : logits_all + static_cast<size_t>(warp) * L.K * CS;
+    float* logits = CTAQ ? logits_all : logits_all + static_cast<size_t>(warp * QPW + half) * L.K * CS;
     float* out_part = logits_all + static_cast<size_t>(L.K) * CS;           // CTAQ only
     const int j0 = CTAQ ? warp : 0, jstep = CTAQ ? kWarps : 1;
 
@@ -99,7 +110,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
     if (PASS >= 1) {
 #pragma unroll
         for (int q = 0; q < CPL; ++q) {
-            const int ch = 32 * q + lane;
+            const int ch = W * q + sl;
 #pragma unroll
             for (int a = 0; a < 3; ++a) w1m[q][a] = __ldg(L.p_w1 + 3 * ch + a);
             b1v[q] = __ldg(L.p_b1 + ch);
@@ -107,23 +118,26 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
     }
     double acc1[PASS == 1 ? CPL : 1], acc2[PASS == 1 ? CPL : 1];         // pass 1: per-lane channel sums
     double sp1[3] = {0.0, 0.0, 0.0}, sp2[3] = {0.0, 0.0, 0.0};           // pass 0
-    double sb1[PASS == 2 ? (CS + 31) / 32 : 1], sb2[PASS == 2 ? (CS + 31) / 32 : 1];
+    double sb1[PASS == 2 ? (CS + W - 1) / W : 1], sb2[PASS == 2 ? (CS + W - 1) / W : 1];
     if (PASS == 1) {
 #pragma unroll
         for (int q = 0; q < CPL; ++q) { acc1[q] = 0.0; acc2[q] = 0.0; }
     }
     if (PASS == 2) {
 #pragma unroll
-        for (int q = 0; q < (CS + 31) / 32; ++q) { sb1[q] = 0.0; sb2[q] = 0.0; }
+        for (int q = 0; q < (CS + W - 1) / W; ++q) { sb1[q] = 0.0; sb2[q] = 0.0; }
     }
 
-    for (int i = CTAQ ? blockIdx.x : blockIdx.x * kWarps + warp; i < L.n; i += CTAQ ? gridDim.x : gridDim.x * kWarps) {
+    // the loop runs over warp-uniform first queries i0, so that both halves of a W = 16 warp take the same trip count
+    for (int i0 = CTAQ ? blockIdx.x : (blockIdx.x * kWarps + warp) * QPW; i0 < L.n; i0 += CTAQ ? gridDim.x : gridDim.x * kWarps * QPW) {
+        const bool valid = W == 32 || i0 + half < L.n;         // false: an idle half-warp, computing on the last query, keeping nothing
+        const int i = W == 32 ? i0 : (valid ? i0 + half : L.n - 1);
         const float pix = __ldg(L.p + 3 * static_cast<size_t>(i)), piy = __ldg(L.p + 3 * static_cast<size_t>(i) + 1),
                     piz = __ldg(L.p + 3 * static_cast<size_t>(i) + 2);
         float xq[CPL];
         if (PASS >= 1) {
 #pragma unroll
-            for (int q = 0; q < CPL; ++q) xq[q] = __ldg(L.xq + static_cast<size_t>(i) * C + 32 * q + lane);
+            for (int q = 0; q < CPL; ++q) xq[q] = __ldg(L.xq + static_cast<size_t>(i) * C + W * q + sl);
         }
         float out[PASS == 3 ? CPL : 1];
 
@@ -131,7 +145,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
             if (PASS == 3 && phase == 1) {
                 // softmax over the K neighbours, one column m per lane (strided), in place (nn.Softmax(dim=1), blocks.py:40)
                 if (CTAQ) __syncthreads(); else __syncwarp();
-                for (int m = CTAQ ? tid : lane; m < CS; m += CTAQ ? kWarps * 32 : 32) {
+                for (int m = CTAQ ? tid : sl; m < CS; m += CTAQ ? kWarps * 32 : W) {
                     float mx = -INFINITY;
                     for (int j = 0; j < L.K; ++j) mx = fmaxf(mx, logits[j * CS + m]);
                     float sum = 0.f;
@@ -150,7 +164,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
 #pragma unroll
                 for (int a = 0; a < 3; ++a) t[a] = fmaf(w0m[3 * a + 2], rz, fmaf(w0m[3 * a + 1], ry, fmaf(w0m[3 * a], rx, b0v[a])));
                 if (PASS == 0) {
-                    if (lane == 0) {
+                    if (sl == 0 && valid) {
 #pragma unroll
                         for (int a = 0; a < 3; ++a) { sp1[a] += t[a]; sp2[a] += static_cast<double>(t[a]) * t[a]; }
                     }
@@ -165,7 +179,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
                 if (PASS == 3 && phase == 1) {
 #pragma unroll
                     for (int q = 0; q < CPL; ++q) {
-                        const int ch = 32 * q + lane;
+                        const int ch = W * q + sl;
                         const float v = __ldg(L.xv + static_cast<size_t>(nbr) * C + ch) + pr[q];
                         out[q] = fmaf(v, logits[j * CS + (ch % CS)], out[q]);
                     }
@@ -173,38 +187,40 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
                 }
                 float w0[CPL];
 #pragma unroll
-                for (int q = 0; q < CPL; ++q) w0[q] = (__ldg(L.xk + static_cast<size_t>(nbr) * C + 32 * q + lane) - xq[q]) + pr[q];
+                for (int q = 0; q < CPL; ++q) w0[q] = (__ldg(L.xk + static_cast<size_t>(nbr) * C + W * q + sl) - xq[q]) + pr[q];
                 if (PASS == 1) {
                     // fp64 per element, as passes 0 and 2: fp32 partial sums of w0^2 lose the variance of a channel whose |mean| >> std
+                    if (valid) {
 #pragma unroll
-                    for (int q = 0; q < CPL; ++q) { acc1[q] += w0[q]; acc2[q] = fma(static_cast<double>(w0[q]), static_cast<double>(w0[q]), acc2[q]); }
+                        for (int q = 0; q < CPL; ++q) { acc1[q] += w0[q]; acc2[q] = fma(static_cast<double>(w0[q]), static_cast<double>(w0[q]), acc2[q]); }
+                    }
                     continue;
                 }
                 // c -> c/8: per-lane partial sums over this lane's channels, butterfly, every lane holds all CS values
                 float u[CPL];
 #pragma unroll
-                for (int q = 0; q < CPL; ++q) u[q] = bn_relu(w0[q], ss_a[32 * q + lane]);
+                for (int q = 0; q < CPL; ++q) u[q] = bn_relu(w0[q], ss_a[W * q + sl]);
                 float w1[CS];
 #pragma unroll
                 for (int m = 0; m < CS; ++m) {
                     float part = 0.f;
 #pragma unroll
-                    for (int q = 0; q < CPL; ++q) part = fmaf(__ldg(L.a_w + static_cast<size_t>(m) * C + 32 * q + lane), u[q], part);
+                    for (int q = 0; q < CPL; ++q) part = fmaf(__ldg(L.a_w + static_cast<size_t>(m) * C + W * q + sl), u[q], part);
 #pragma unroll
-                    for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
+                    for (int o = W / 2; o; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
                     w1[m] = part + __ldg(L.a_b + m);
                 }
                 if (PASS == 2) {
 #pragma unroll
                     for (int m = 0; m < CS; ++m)
-                        if (lane == (m & 31)) { sb1[m >> 5] += w1[m]; sb2[m >> 5] += static_cast<double>(w1[m]) * w1[m]; }
+                        if (sl == (m & (W - 1)) && valid) { sb1[m / W] += w1[m]; sb2[m / W] += static_cast<double>(w1[m]) * w1[m]; }
                     continue;
                 }
                 // PASS 3, phase 0: second small product, logits to shared memory
                 float v1[CS];
 #pragma unroll
                 for (int m = 0; m < CS; ++m) v1[m] = bn_relu(w1[m], ss_b[m]);
-                for (int mo = lane; mo < CS; mo += 32) {
+                for (int mo = sl; mo < CS; mo += W) {
                     float s = __ldg(L.b_b + mo);
 #pragma unroll
                     for (int m = 0; m < CS; ++m) s = fmaf(__ldg(L.b_w + static_cast<size_t>(mo) * CS + m), v1[m], s);
@@ -213,8 +229,10 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
             }
         }
         if (PASS == 3 && !CTAQ) {
+            if (valid) {
 #pragma unroll
-            for (int q = 0; q < CPL; ++q) L.out[static_cast<size_t>(i) * C + 32 * q + lane] = out[q];
+                for (int q = 0; q < CPL; ++q) L.out[static_cast<size_t>(i) * C + W * q + sl] = out[q];
+            }
             __syncwarp();                                          // the next query's logits overwrite the weights read above
         }
         if (PASS == 3 && CTAQ) {
@@ -231,6 +249,19 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
         }
     }
     if (PASS == 1 || PASS == 2) __syncthreads();                   // the statistics below reuse the logits area
+    if constexpr (W == 16) {
+        // lanes l and l + 16 hold sums of the same channels (of two queries): fold the upper half into the lower before the CTA sum
+#pragma unroll
+        for (int a = 0; a < 3; ++a) { sp1[a] += __shfl_xor_sync(FULL, sp1[a], 16); sp2[a] += __shfl_xor_sync(FULL, sp2[a], 16); }
+        if (PASS == 1) {
+#pragma unroll
+            for (int q = 0; q < CPL; ++q) { acc1[q] += __shfl_xor_sync(FULL, acc1[q], 16); acc2[q] += __shfl_xor_sync(FULL, acc2[q], 16); }
+        }
+        if (PASS == 2) {
+#pragma unroll
+            for (int q = 0; q < (CS + W - 1) / W; ++q) { sb1[q] += __shfl_xor_sync(FULL, sb1[q], 16); sb2[q] += __shfl_xor_sync(FULL, sb2[q], 16); }
+        }
+    }
 
     // ---- statistics: CTA reduction, two fp64 atomics per channel per CTA --------------------------------------------------
     if (PASS == 0) {
@@ -249,8 +280,10 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
         double* sh = reinterpret_cast<double*>(logits_all);      // [kWarps][2][C] doubles (the logits area is idle in this pass)
 #pragma unroll
         for (int q = 0; q < CPL; ++q) {
-            sh[(warp * 2) * C + 32 * q + lane] = acc1[q];
-            sh[(warp * 2 + 1) * C + 32 * q + lane] = acc2[q];
+            if (lane < W) {
+                sh[(warp * 2) * C + W * q + lane] = acc1[q];
+                sh[(warp * 2 + 1) * C + W * q + lane] = acc2[q];
+            }
         }
         __syncthreads();
         for (int e = tid; e < 2 * C; e += kWarps * 32) {
@@ -264,7 +297,7 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
         double* sh = reinterpret_cast<double*>(logits_all);      // [kWarps][2][CS]
 #pragma unroll
         for (int m = 0; m < CS; ++m)
-            if (lane == (m & 31)) { sh[(warp * 2) * CS + m] = sb1[m >> 5]; sh[(warp * 2 + 1) * CS + m] = sb2[m >> 5]; }
+            if (lane == (m & (W - 1))) { sh[(warp * 2) * CS + m] = sb1[m / W]; sh[(warp * 2 + 1) * CS + m] = sb2[m / W]; }
         __syncthreads();
         for (int e = tid; e < 2 * CS; e += kWarps * 32) {
             const int which = e / CS, m = e - which * CS;
@@ -294,38 +327,41 @@ __global__ void pt_update_running_kernel(const tgn_pt_layer_t L)
     }
 }
 
-template <int CPL, int PASS, bool CTAQ>
+template <int CPL, int PASS, bool CTAQ, int W = 32>
 int launch_pass_as(const tgn_pt_layer_t& L, cudaStream_t st)
 {
-    constexpr int C = 32 * CPL, CS = 4 * CPL;
+    constexpr int C = W * CPL, CS = C / 8, QPW = 32 / W;
     const size_t head = (C + CS + 4) * sizeof(BnAffine);
-    size_t smem = head + static_cast<size_t>(kWarps) * L.K * CS * sizeof(float);
+    size_t smem = head + static_cast<size_t>(kWarps) * QPW * L.K * CS * sizeof(float);
     smem = std::max(smem, head + static_cast<size_t>(kWarps) * 2 * C * sizeof(double));
     smem = std::max(smem, head + (static_cast<size_t>(L.K) * CS + static_cast<size_t>(kWarps) * C) * sizeof(float));
-    const int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(pt_layer_kernel<CPL, PASS, CTAQ>), smem);
+    const int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(pt_layer_kernel<CPL, PASS, CTAQ, W>), smem);
     if (rc != TGN_OK) return rc;
-    const int grid = CTAQ ? std::max(1, std::min(L.n, 8 * sm_count())) : std::max(1, std::min((L.n + kWarps - 1) / kWarps, 4 * sm_count()));
-    pt_layer_kernel<CPL, PASS, CTAQ><<<grid, kWarps * 32, smem, st>>>(L);
+    const int per_cta = CTAQ ? 1 : kWarps * QPW;
+    const int grid = std::max(1, std::min((L.n + per_cta - 1) / per_cta, (CTAQ ? 8 : 4) * sm_count()));
+    pt_layer_kernel<CPL, PASS, CTAQ, W><<<grid, kWarps * 32, smem, st>>>(L);
     return check_launch("pt_layer_kernel");
 }
 
 // queries below this count get a CTA each (0 = never, INT_MAX = always: tgn_pt_layer_set_cta_threshold, for measurements)
 int g_cta_threshold = 1024;
 
-template <int CPL, int PASS>
+// c = 16 (W = 16) always runs two queries per warp: the threshold does not apply to it
+template <int CPL, int PASS, int W>
 int launch_pass(const tgn_pt_layer_t& L, cudaStream_t st)
 {
-    return L.n < g_cta_threshold ? launch_pass_as<CPL, PASS, true>(L, st) : launch_pass_as<CPL, PASS, false>(L, st);
+    if constexpr (W == 16) return launch_pass_as<CPL, PASS, false, 16>(L, st);
+    else return L.n < g_cta_threshold ? launch_pass_as<CPL, PASS, true>(L, st) : launch_pass_as<CPL, PASS, false>(L, st);
 }
 
-template <int CPL>
+template <int CPL, int W = 32>
 int run_layer(const tgn_pt_layer_t& L, cudaStream_t st)
 {
     int rc = TGN_OK;
-    if (L.bn_mode[0] == 1 && (rc = launch_pass<CPL, 0>(L, st)) != TGN_OK) return rc;
-    if (L.bn_mode[1] == 1 && (rc = launch_pass<CPL, 1>(L, st)) != TGN_OK) return rc;
-    if (L.bn_mode[2] == 1 && (rc = launch_pass<CPL, 2>(L, st)) != TGN_OK) return rc;
-    if ((rc = launch_pass<CPL, 3>(L, st)) != TGN_OK) return rc;
+    if (L.bn_mode[0] == 1 && (rc = launch_pass<CPL, 0, W>(L, st)) != TGN_OK) return rc;
+    if (L.bn_mode[1] == 1 && (rc = launch_pass<CPL, 1, W>(L, st)) != TGN_OK) return rc;
+    if (L.bn_mode[2] == 1 && (rc = launch_pass<CPL, 2, W>(L, st)) != TGN_OK) return rc;
+    if ((rc = launch_pass<CPL, 3, W>(L, st)) != TGN_OK) return rc;
     if (L.update_running) {
         pt_update_running_kernel<<<(3 + L.c + L.c / 8 + 127) / 128, 128, 0, st>>>(L);
         rc = check_launch("pt_update_running_kernel");
@@ -353,7 +389,7 @@ int tgn_pt_layer_forward(const tgn_pt_layer_t* layer, void* stream)
     if (!layer) { set_error("pt_layer_forward: null descriptor"); return TGN_ERR_INVALID; }
     const tgn_pt_layer_t& L = *layer;
     if (L.n <= 0) return TGN_OK;
-    if (L.K < 1 || L.K > 64 || !(L.c == 32 || L.c == 64 || L.c == 128 || L.c == 256 || L.c == 512)) {
+    if (L.K < 1 || L.K > 64 || !(L.c == 16 || L.c == 32 || L.c == 64 || L.c == 128 || L.c == 256 || L.c == 512)) {
         set_error("pt_layer_forward: unsupported shape c=%d K=%d", L.c, L.K);
         return TGN_ERR_INVALID;
     }
@@ -361,6 +397,7 @@ int tgn_pt_layer_forward(const tgn_pt_layer_t* layer, void* stream)
         !L.stats_p || !L.stats_a || !L.stats_b) { set_error("pt_layer_forward: null argument"); return TGN_ERR_INVALID; }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     switch (L.c) {
+        case 16: return run_layer<1, 16>(L, st);
         case 32: return run_layer<1>(L, st);
         case 64: return run_layer<2>(L, st);
         case 128: return run_layer<4>(L, st);
