@@ -50,8 +50,13 @@ def _pack(cl, ms):
     return xyz, offset, new_offset
 
 
+# 100*G + CS; -(40 + W): single-barrier bucket schedule; -(80 + W): + register-resident tables (shared-memory tables when a cloud has
+# more buckets per lane than the registers hold)
+FPS_MODES = [0, 1, 2, 4, 8, 201, 202, 204, 208, -1, -2, -3, -42, -44, -48, -56, -72, -84, -88, -96, -112]
+
+
 @pytest.mark.parametrize("name,build,ms", FPS_CASES, ids=[c[0] for c in FPS_CASES])
-@pytest.mark.parametrize("mode", [0, 1, 2, 4, 8, 201, 202, 204, 208, -1, -2, -3, -42, -44, -48, -56, -72, -84, -88, -96, -112])   # 100*G + CS; -(40 + W): single-barrier bucket schedule; -(80 + W): + register-resident tables (shared-memory tables when a cloud has more buckets per lane than the registers hold)
+@pytest.mark.parametrize("mode", FPS_MODES)
 def test_fps_matches_oracle(name, build, ms, mode):
     cl = build()
     xyz, offset, new_offset = _pack(cl, ms)

@@ -378,8 +378,9 @@ const FpsConfig kConfigs[] = {
     {512, 4, 2, 1}, {512, 8, 2, 1}, {512, 12, 2, 1}, {512, 16, 2, 1}, {512, 24, 2, 1},
     {512, 4, 4, 1}, {512, 8, 4, 1}, {512, 12, 4, 1}, {512, 16, 4, 1}, {512, 24, 4, 1},
     {512, 4, 8, 1}, {512, 8, 8, 1}, {512, 12, 8, 1}, {512, 16, 8, 1}, {512, 24, 8, 1},
-    // software-pipelined: two clouds per cluster
-    {512, 4, 1, 2}, {512, 8, 1, 2}, {512, 12, 1, 2},
+    // software-pipelined: two clouds per cluster (one CTA of 512 threads holds no cloud past 1 023 points, where the block size
+    // of the tie order reaches 1 024, so only the smallest single-CTA shape is ever picked)
+    {512, 4, 1, 2},
     {512, 4, 2, 2}, {512, 8, 2, 2}, {512, 12, 2, 2},
     {512, 4, 4, 2}, {512, 8, 4, 2}, {512, 12, 4, 2},
     {512, 8, 8, 2}, {512, 12, 8, 2},
@@ -414,7 +415,7 @@ int dispatch_resident(const FpsConfig& c, int b, const float* xyz, const int* of
     TGN_FPS_CASE(512, 24, 4, 1)
     TGN_FPS_CASE(512, 4, 8, 1) TGN_FPS_CASE(512, 8, 8, 1) TGN_FPS_CASE(512, 12, 8, 1) TGN_FPS_CASE(512, 16, 8, 1)
     TGN_FPS_CASE(512, 24, 8, 1)
-    TGN_FPS_CASE(512, 4, 1, 2) TGN_FPS_CASE(512, 8, 1, 2) TGN_FPS_CASE(512, 12, 1, 2)
+    TGN_FPS_CASE(512, 4, 1, 2)
     TGN_FPS_CASE(512, 4, 2, 2) TGN_FPS_CASE(512, 8, 2, 2) TGN_FPS_CASE(512, 12, 2, 2)
     TGN_FPS_CASE(512, 4, 4, 2) TGN_FPS_CASE(512, 8, 4, 2) TGN_FPS_CASE(512, 12, 4, 2)
     TGN_FPS_CASE(512, 8, 8, 2) TGN_FPS_CASE(512, 12, 8, 2)
@@ -424,11 +425,17 @@ int dispatch_resident(const FpsConfig& c, int b, const float* xyz, const int* of
 
 }  // namespace
 
-// mode: 0 auto, -1 streaming kernel, -2 bucket-pruned kernel, otherwise 100*G + CS (G omitted = 1):
-// force that register-resident shape.
+// mode: 0 auto, -1 streaming kernel, -2 bucket-pruned kernel, -3 / -(10 + W) / -(40 + W) / -(80 + W) bucket kernel
+// schedules (below), otherwise 100*G + CS (G omitted = 1): force that register-resident shape.  Any other negative mode
+// is refused, and so is a bucket shape without a kernel, before anything is launched.
 int fps_dispatch(int b, int n_max, const float* xyz, const int* offset, const int* new_offset, float* tmp, int* idx,
                  int mode, cudaStream_t stream)
 {
+    // A mode outside the documented set is refused rather than run as auto: a mistyped mode must not quietly test another kernel.
+    if (mode < 0 && !(mode >= -3 || (mode <= -11 && mode >= -26) || (mode <= -41 && mode >= -72) || (mode <= -81 && mode >= -112))) {
+        set_error("furthestsampling: unknown mode %d", mode);
+        return TGN_ERR_INVALID;
+    }
     if (b <= 0) return TGN_OK;
     if (n_max <= 0) { set_error("furthestsampling: n_max must be positive"); return TGN_ERR_INVALID; }
     const int bs_log2 = ref_block_log2(n_max);

@@ -877,6 +877,35 @@ int fps_bucket_launch(int b, int n_max, const float* xyz, const int* offset, con
     BucketWs ws{};
     ws.stride = (n_max + kBP - 1) / kBP * kBP;
     ws.nbmax = ws.stride / kBP;
+    // The main kernel's shape is decided before anything is allocated or launched: a refused shape launches nothing.
+    const size_t smem = static_cast<size_t>(ws.nbmax) * (sizeof(float4) * 3 + sizeof(int));
+    // Warps per cloud by batch size: the more clouds per SM are available, the narrower the CTA (fewer
+    // redundant per-warp steps and cheaper barriers per cloud, more clouds in flight to hide latency).
+    const int sms = sm_count();
+    auto fits = [&](int per_sm) { return static_cast<size_t>(per_sm) * (smem + 1024) <= 220 * 1024; };
+    // Auto (shape 0), 24k-point clouds -> 1024 samples: up to 4 clouds per SM the single-barrier kernel with register-resident
+    // tables at 16 warps per cloud; beyond that the batch is DRAM-bound and the three-barrier kernel at 4 warps per cloud,
+    // 8 clouds per SM, is used.
+    // Raw meshes (one cloud of 1e5..2e5 vertices -> 24 000, gen_utils.py:135-140): the same kernel with 4-8 buckets per lane
+    // while every cloud can have an SM to itself.
+    if (shape == 0 && ((b <= 4 * sms && ws.nbmax <= 2 * 512) || (b <= sms && ws.nbmax <= 8 * 512))) shape = 200 + 16;
+    const bool v2 = shape >= 100 && shape < 200;          // 100 + W: the single-barrier schedule (fps_bucket_kernel2)
+    const bool v3 = shape >= 200;                         // 200 + W: the same with register-resident bucket tables (fps_bucket_kernel3)
+    int warps = shape % 100;
+    if (warps == 0) warps = (b > 4 * sms && fits(8)) ? 4 : (b > 2 * sms && fits(4)) ? 8 : 16;
+    if (v3 && warps != 32 && warps != 16 && warps != 8 && warps != 4) {
+        set_error("furthestsampling: bucket kernel v3 has no shape of %d warps per cloud", warps);
+        return TGN_ERR_INVALID;
+    }
+    if (v2 && warps != 32 && warps != 16 && warps != 8 && warps != 4 && warps != 2) {
+        set_error("furthestsampling: bucket kernel v2 has no shape of %d warps per cloud", warps);
+        return TGN_ERR_INVALID;
+    }
+    if (!v2 && !v3 && warps != 16 && warps != 8 && warps != 4 && warps != 2 && warps != 1) {
+        set_error("furthestsampling: bucket kernel has no shape of %d warps per cloud", warps);
+        return TGN_ERR_INVALID;
+    }
+
     const bool smem_sort = n_max <= kSmemSortMaxN;
     const size_t pts = static_cast<size_t>(b) * ws.stride;
     const size_t nbt = static_cast<size_t>(b) * ws.nbmax;
@@ -910,21 +939,7 @@ int fps_bucket_launch(int b, int n_max, const float* xyz, const int* offset, con
     }
     int rc = check_launch("fps_bucket_sort_kernel");
     if (rc == TGN_OK) {
-        const size_t smem = static_cast<size_t>(ws.nbmax) * (sizeof(float4) * 3 + sizeof(int));
-        // Warps per cloud by batch size: the more clouds per SM are available, the narrower the CTA (fewer
-        // redundant per-warp steps and cheaper barriers per cloud, more clouds in flight to hide latency).
-        const int sms = sm_count();
-        auto fits = [&](int per_sm) { return static_cast<size_t>(per_sm) * (smem + 1024) <= 220 * 1024; };
-        // Auto (shape 0), 24k-point clouds -> 1024 samples: up to 4 clouds per SM the single-barrier kernel with register-resident
-        // tables at 16 warps per cloud; beyond that the batch is DRAM-bound and the three-barrier kernel at 4 warps per cloud,
-        // 8 clouds per SM, is used.
-        // Raw meshes (one cloud of 1e5..2e5 vertices -> 24 000, gen_utils.py:135-140): the same kernel with 4-8 buckets per lane
-        // while every cloud can have an SM to itself.
-        if (shape == 0 && ((b <= 4 * sms && ws.nbmax <= 2 * 512) || (b <= sms && ws.nbmax <= 8 * 512))) shape = 200 + 16;
-        const bool v2 = shape >= 100 && shape < 200;          // 100 + W: the single-barrier schedule (fps_bucket_kernel2)
-        const bool v3 = shape >= 200;                         // 200 + W: the same with register-resident bucket tables (fps_bucket_kernel3)
-        int warps = shape % 100;
-        if (warps == 0) warps = (b > 4 * sms && fits(8)) ? 4 : (b > 2 * sms && fits(4)) ? 8 : 16;
+        // every (kernel, warps) pair below was admitted above
         if (v3) {
             const int bpl = (ws.nbmax + warps * 32 - 1) / (warps * 32);          // buckets per lane
             rc = -1;
