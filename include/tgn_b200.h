@@ -129,6 +129,19 @@ int tgn_kmeans(int B, long long n_total, int k, int max_iter, const int *offsets
 int tgn_meanshift(int n, int n_nodes, const double *Xt, const long long *idx, const int *nodes, const double *bounds, double bandwidth,
                   double stop_thresh, int max_iter, double *means, int *info, void *stream);
 
+/* scikit-learn 1.9's KDTree(xyz, leaf_size) built on the device, bit for bit: the arrays of KDTree.get_arrays() for float64
+ * (n,3) points (the label transfers' tie fallback, MeanShift's tree).  tgn_kdtree_nodes(n, leaf_size) = n_nodes
+ * (2^n_levels - 1, -1 for arguments out of range); a DEVICE workspace of tgn_kdtree_bytes(n, leaf_size) bytes.  Outputs,
+ * DEVICE: idx_array (n) int64; node_data (n_nodes) records of scikit-learn's NodeData_t {idx_start, idx_end, is_leaf int64;
+ * radius float64}, the radius left NaN; node_bounds (2, n_nodes, 3) float64.  No host synchronisation.  1 <= n <= 2^30,
+ * finite coordinates (not checked here), leaf_size >= 1.  tgn_kdtree_radius fills the radius of HOST copies of node_data from
+ * node_bounds the way scikit-learn's init_node computes it, with the C library's pow. */
+int tgn_kdtree_nodes(int n, int leaf_size);
+size_t tgn_kdtree_bytes(int n, int leaf_size);
+int tgn_kdtree_build(int n, int leaf_size, const double *xyz, long long *idx_array, long long *node_data, double *node_bounds,
+                     void *workspace, void *stream);
+void tgn_kdtree_radius(int n_nodes, const double *node_bounds, double *node_data);
+
 /* Exact float64 kNN with a fused label vote: the answer of sklearn KDTree(xyz).query(queries, k) -- boundary detection of
  * InferencePipeLine.get_boundary_sampled_feats (inference_pipeline_tgn.py:289-330).  xyz (n,3) and queries (m,3) float64
  * DEVICE; 1 <= k <= 64, k <= n.  Distances d2 = (dx*dx + dy*dy) + dz*dz in float64 without contraction, neighbours ascending

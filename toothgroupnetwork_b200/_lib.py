@@ -61,6 +61,7 @@ _SIGS = {
                                _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp],
     "tgn_kmeans": [_i, ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_meanshift": [_i, _i, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _i, _vp, _vp, _vp],
+    "tgn_kdtree_build": [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp],
 }
 
 
@@ -120,7 +121,7 @@ REFERENCE_LAUNCHERS = [
     "subtraction_forward_cuda_launcher", "subtraction_backward_cuda_launcher",
     "aggregation_forward_cuda_launcher", "aggregation_backward_cuda_launcher",
 ]
-EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes"]
+EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes", "tgn_kdtree_nodes", "tgn_kdtree_bytes", "tgn_kdtree_radius"]
 
 
 class TgnError(RuntimeError):
@@ -156,6 +157,12 @@ def load() -> ctypes.CDLL:
     lib.tgn_knn_f64_bytes.restype = ctypes.c_size_t
     lib.tgn_kmeans_bytes.argtypes = [ctypes.c_longlong, _i]
     lib.tgn_kmeans_bytes.restype = ctypes.c_size_t
+    lib.tgn_kdtree_nodes.argtypes = [_i, _i]
+    lib.tgn_kdtree_nodes.restype = _i
+    lib.tgn_kdtree_bytes.argtypes = [_i, _i]
+    lib.tgn_kdtree_bytes.restype = ctypes.c_size_t
+    lib.tgn_kdtree_radius.argtypes = [_i, _vp, _vp]
+    lib.tgn_kdtree_radius.restype = None
     lib.tgn_pw_struct_size.argtypes = [_i]
     lib.tgn_pw_struct_size.restype = _i
     lib.tgn_pt_layer_struct_size.restype = _i

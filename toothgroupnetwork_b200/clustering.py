@@ -23,6 +23,7 @@ import torch
 
 from . import _lib as L
 from . import crops
+from . import neighbors
 
 _ws = {}
 
@@ -344,7 +345,8 @@ def meanshift_unpack(buf: np.ndarray):
 
 def meanshift_tree(X: np.ndarray):
     """scikit-learn's ``KDTree(X, leaf_size=30)`` (the tree ``NearestNeighbors(radius=...).fit(X)`` builds for n >= 12) as the
-    kernel's arrays: (Xt, idx_array, nodes (n_nodes,3) int32, node_bounds)."""
+    kernel's arrays: (Xt, idx_array, nodes (n_nodes,3) int32, node_bounds), built by scikit-learn on the host -- the reference
+    the device build of ``MeanShift.fit`` is tested against."""
     from sklearn.neighbors import KDTree
     _, idx, node_data, bounds = KDTree(X, leaf_size=_MS_LEAF_SIZE).get_arrays()
     nodes = np.stack([node_data["idx_start"], node_data["idx_end"], node_data["is_leaf"]], axis=1).astype(np.int32)
@@ -400,8 +402,8 @@ class MeanShift:
     ``.labels_`` (ops_utils.py:130 in ``get_clustering_labels``), plus ``.cluster_centers_`` / ``.n_iter_`` -- with the seed
     ascent on csrc/meanshift.cu, on float64 (n, 3) points.
 
-    The host builds scikit-learn's own KD tree (milliseconds) and hands the kernel its arrays; every seed climbs on the device
-    with scikit-learn's float64 rounding.  Seeds the kernel flags (a distance or a step within 2^-40 relative of the radius or
+    scikit-learn's own ``KDTree(X, leaf_size=30)`` is built on the device (``neighbors.sklearn_tree``, bit for bit) and stays
+    there; every seed climbs on the device with scikit-learn's float64 rounding.  Seeds the kernel flags (a distance or a step within 2^-40 relative of the radius or
     the stop threshold, where scikit-learn's node bounds or another BLAS order could decide otherwise) are redone with
     scikit-learn's public calls and counted in ``host_seeds``.  The post-processing is scikit-learn's, so cluster_centers_,
     labels_ and n_iter_ are its own.  Inputs of at most 11 points, which scikit-learn searches by brute force, go to scikit-learn
@@ -439,9 +441,9 @@ class MeanShift:
             return self
         if not torch.cuda.is_available():
             raise L.TgnError("MeanShift needs a CUDA device (there is no CPU path)")
-        Xt, idx, nodes, bounds = meanshift_tree(X)
-        dev = [torch.from_numpy(a).cuda() for a in (Xt, idx, nodes, bounds)]
-        means, counts, iters, flags = meanshift_unpack(meanshift_device(*dev, r, self.max_iter).cpu().numpy())
+        xyz, idx, node_data, bounds = neighbors.sklearn_tree(X, _MS_LEAF_SIZE, radius=False)
+        tree = (xyz[idx], idx, node_data[:, :3].int(), bounds)
+        means, counts, iters, flags = meanshift_unpack(meanshift_device(*tree, r, self.max_iter).cpu().numpy())
         flagged = np.flatnonzero(flags)
         if flagged.size:
             from sklearn.neighbors import NearestNeighbors

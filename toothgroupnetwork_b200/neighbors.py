@@ -6,10 +6,14 @@ and :137-140, inference_pipeline_tsegnet.py:72-74, inference_pipeline_sem.py:37-
 of csrc/knn_f64.cu once per point set and answers every ``query`` with one upload, one launch and one download.
 
 The kernel's neighbours are ordered by (d2, index), while the KDTree keeps whichever exactly tied point its depth-first walk
-meets first -- an order set by its in-leaf layout, which the GPU cannot reproduce.  So each query also returns a tie flag: a row
-whose min(k+1, n) best squared distances are all distinct has one answer under any tie-break rule and is taken from the GPU; the
-flagged rows are re-answered by scikit-learn's own tree, built on the first flag and kept.  Duplicated vertices make such rows
-common (a point that is both an FPS sample and a kept boundary vertex is in tgn's final tree twice).  ``host_rows`` counts them.
+meets first -- an order set by its in-leaf layout.  So each query also returns a tie flag: a row whose min(k+1, n) best squared
+distances are all distinct has one answer under any tie-break rule and is taken from the GPU; the flagged rows are re-answered
+by scikit-learn's own query code.  Duplicated vertices make such rows common (a point that is both an FPS sample and a kept
+boundary vertex is in tgn's final tree twice).  ``host_rows`` counts them.
+
+The tree those rows need is scikit-learn's, bit for bit, and ``sklearn_tree`` builds it on the device (csrc/kdtree_build.cu,
+DESIGN §3.16): on the first flagged row its arrays are copied to the host once and a scikit-learn ``KDTree`` is restored from
+them with ``__setstate__``, without a host build.  An installation whose pickled state has another layout builds it on the host.
 
 ``accelerate(module)`` points a module's ``KDTree`` name at the class.  scikit-learn is imported only when a row is flagged.
 """
@@ -123,14 +127,138 @@ class KDTree:
         rows = np.flatnonzero(host[n_idx + n_dist:])
         if rows.size:
             if self._host_tree is None:
-                from sklearn.neighbors import KDTree as HostKDTree
-                self._host_tree = HostKDTree(self._X, leaf_size=self.leaf_size)
+                self._host_tree = host_tree(self._X, self._xyz, self.leaf_size)
             self.host_rows += int(rows.size)
             if return_distance:
                 d[rows], ind[rows] = self._host_tree.query(X[rows], k=k)
             else:
                 ind[rows] = self._host_tree.query(X[rows], k=k, return_distance=False)
         return (d, ind) if return_distance else ind
+
+
+NODE_DATA = np.dtype([("idx_start", "<i8"), ("idx_end", "<i8"), ("is_leaf", "<i8"), ("radius", "<f8")])   # NodeData_t
+
+
+def tree_nodes(n: int, leaf_size: int) -> int:
+    """scikit-learn's node count: 2^n_levels - 1 with n_levels = int(log2(max(1, (n - 1) / leaf_size)) + 1)"""
+    n_levels = int(np.log2(max(1.0, (n - 1) / leaf_size)) + 1)
+    return 2 ** n_levels - 1
+
+
+def _device_points(X) -> torch.Tensor:
+    """(n, 3) float64 finite points -> a contiguous CUDA tensor, refused (ValueError, as scikit-learn) before any launch"""
+    if torch.is_tensor(X):
+        L.require_cuda(X)
+        if X.dim() != 2 or X.shape[1] != 3 or X.dtype != torch.float64:
+            raise L.TgnError(f"sklearn_tree: expected (n, 3) float64 points, got {tuple(X.shape)} {X.dtype}")
+        if X.shape[0] == 0:
+            raise ValueError("X is an empty array")
+        if not bool(torch.isfinite(X).all()):
+            raise ValueError("Input contains NaN or infinity.")
+        return X.contiguous()
+    X = _as_points(X)
+    if X.shape[1] != 3:
+        raise L.TgnError(f"sklearn_tree: only (n, 3) points are implemented, got {X.shape}")
+    if not torch.cuda.is_available():
+        raise L.TgnError("sklearn_tree needs a CUDA device (there is no CPU path)")
+    return torch.from_numpy(X).cuda()
+
+
+def _build(xyz: torch.Tensor, leaf_size: int):
+    """csrc/kdtree_build.cu on the current stream -> (idx_array int64 (n), node_data int64 (n_nodes, 4) with the radius
+    column NaN, node_bounds float64 (2, n_nodes, 3)), all on xyz's device"""
+    if isinstance(leaf_size, bool) or not isinstance(leaf_size, (int, np.integer)) or leaf_size < 1:
+        raise ValueError("leaf_size must be greater than or equal to 1")
+    n = int(xyz.shape[0])
+    n_nodes = tree_nodes(n, int(leaf_size))
+    if int(L.load().tgn_kdtree_nodes(n, int(leaf_size))) != n_nodes:
+        raise L.TgnError(f"sklearn_tree: n={n} leaf_size={leaf_size} is outside the device build's range")
+    dev = xyz.device
+    idx = torch.empty(n, dtype=torch.int64, device=dev)
+    node_data = torch.empty((n_nodes, 4), dtype=torch.int64, device=dev)
+    bounds = torch.empty((2, n_nodes, 3), dtype=torch.float64, device=dev)
+    ws = torch.empty(int(L.load().tgn_kdtree_bytes(n, int(leaf_size))), dtype=torch.uint8, device=dev)
+    L.call("tgn_kdtree_build", n, int(leaf_size), L.ptr(xyz), L.ptr(idx), L.ptr(node_data), L.ptr(bounds), L.ptr(ws),
+           L.stream_ptr())
+    return idx, node_data, bounds
+
+
+def _fill_radius(node_data: np.ndarray, bounds: np.ndarray) -> None:
+    """init_node's radius into host node_data (n_nodes, 4) 8-byte records from host node_bounds, with the C library's pow as
+    scikit-learn computes it (the device's correctly rounded sqrt and squares differ from it in about 1 node in 1000)"""
+    L.load().tgn_kdtree_radius(int(node_data.shape[0]), bounds.ctypes.data, node_data.ctypes.data)
+
+
+def sklearn_tree(X, leaf_size: int = 40, radius: bool = True):
+    """``sklearn.neighbors.KDTree(X, leaf_size).get_arrays()`` built on the GPU, bit for bit: (data (n,3) float64,
+    idx_array int64 (n), node_data int64 (n_nodes, 4) = NodeData_t's idx_start, idx_end, is_leaf and the float64 bits of
+    radius, node_bounds float64 (2, n_nodes, 3)), all on the device.  X is host (n, 3) points or a float64 CUDA tensor; empty,
+    non-finite input and leaf_size < 1 are refused with scikit-learn's ValueError before any launch.  The radius is computed
+    on the host from the bounds (one copy each way); with ``radius=False`` it stays NaN and nothing leaves the device.
+    ``node_data.cpu().numpy().view(NODE_DATA)`` is scikit-learn's record array."""
+    if isinstance(leaf_size, bool) or not isinstance(leaf_size, (int, np.integer)) or leaf_size < 1:
+        raise ValueError("leaf_size must be greater than or equal to 1")
+    xyz = _device_points(X)
+    idx, node_data, bounds = _build(xyz, leaf_size)
+    if not radius:
+        return xyz, idx, node_data, bounds
+    host_bounds = bounds.cpu().numpy()
+    host_nodes = node_data.cpu().numpy()
+    _fill_radius(host_nodes, host_bounds)
+    node_data[:, 3].copy_(torch.from_numpy(np.ascontiguousarray(host_nodes[:, 3])))
+    return xyz, idx, node_data, bounds
+
+
+def host_kdtree_class():
+    """The host class the tie fallback restores (or, on an unexpected state layout, builds): scikit-learn's KDTree."""
+    from sklearn.neighbors import KDTree as HostKDTree
+    return HostKDTree
+
+
+_state_ok = None
+
+
+def _state_layout_ok(cls) -> bool:
+    """Whether this scikit-learn pickles a KDTree the way 1.9 does: 13 fields, float64 data, intp idx_array, NodeData_t
+    records, float64 bounds, a Euclidean metric object -- checked once on an empty instance, without a build."""
+    global _state_ok
+    if _state_ok is None:
+        try:
+            st = cls.__new__(cls).__getstate__()
+            from sklearn.metrics import DistanceMetric
+            metric = DistanceMetric.get_metric("minkowski", p=2)
+            _state_ok = (len(st) == 13 and st[0].dtype == np.float64 and st[1].dtype == np.intp and st[2].dtype == NODE_DATA
+                         and st[3].dtype == np.float64 and st[3].ndim == 3 and type(metric).__name__ == "EuclideanDistance64")
+        except Exception:
+            _state_ok = False
+    return _state_ok
+
+
+def host_tree(X: np.ndarray, xyz: torch.Tensor, leaf_size: int):
+    """scikit-learn's ``KDTree(X, leaf_size)`` for host queries: built on the device from xyz (X on the device), copied once
+    and restored with ``__setstate__``; built on the host when this scikit-learn's state layout is not the expected one."""
+    cls = host_kdtree_class()
+    if not _state_layout_ok(cls) or isinstance(leaf_size, bool) or not isinstance(leaf_size, (int, np.integer)):
+        return cls(X, leaf_size=leaf_size)
+    idx, node_data, bounds = _build(xyz, leaf_size)
+    n, n_nodes = idx.numel(), node_data.shape[0]
+    flat = torch.cat([idx, node_data.reshape(-1), bounds.reshape(-1).view(torch.int64)]).cpu().numpy()   # one copy
+    idx_h = flat[:n].astype(np.intp, copy=False)
+    nodes_h = np.ascontiguousarray(flat[n:n + 4 * n_nodes]).reshape(n_nodes, 4)
+    bounds_h = np.ascontiguousarray(flat[n + 4 * n_nodes:]).view(np.float64).reshape(2, n_nodes, 3)
+    _fill_radius(nodes_h, bounds_h)
+    return restore(cls, X, idx_h, nodes_h.view(NODE_DATA).reshape(n_nodes), bounds_h, leaf_size)
+
+
+def restore(cls, X: np.ndarray, idx_array: np.ndarray, node_data: np.ndarray, node_bounds: np.ndarray, leaf_size: int):
+    """A scikit-learn KDTree of class ``cls`` from the arrays ``get_arrays()`` returns, by ``__setstate__`` (no build): the
+    state of a freshly built tree -- no query counters, the Euclidean metric, no sample weights."""
+    from sklearn.metrics import DistanceMetric
+    n_nodes = int(node_data.shape[0])
+    tree = cls.__new__(cls)
+    tree.__setstate__((X, idx_array, node_data, node_bounds, int(leaf_size), int(np.log2(n_nodes + 1)), n_nodes, 0, 0, 0, 0,
+                       DistanceMetric.get_metric("minkowski", p=2), None))
+    return tree
 
 
 def accelerate(module) -> None:
