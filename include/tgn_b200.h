@@ -142,6 +142,18 @@ int tgn_kdtree_build(int n, int leaf_size, const double *xyz, long long *idx_arr
                      void *workspace, void *stream);
 void tgn_kdtree_radius(int n_nodes, const double *node_bounds, double *node_data);
 
+/* scikit-learn 1.9's KDTree.query(queries, k) (single tree, depth first, sorted results) over the arrays tgn_kdtree_build
+ * writes, one warp per row.  xyz (n,3) float64 in original order, idx_array (n) int64, node_data (n_nodes,4) int64 (the radius
+ * is not read), node_bounds (2,n_nodes,3) float64, queries (m,3) float64 finite, all DEVICE.  rows (n_rows) int64 DEVICE row
+ * numbers, or NULL for every row; only the listed rows of the outputs are written (a number outside [0, m) is skipped).
+ * Outputs, DEVICE: idx (m,k) int64; dist (m,k) float64 = sqrt of the reduced distance, optional (NULL); flag (m) bytes: 1 when a
+ * trim or child-order decision compared a node bound whose squares were not all exact within a relative 2^-40 (only there may
+ * scikit-learn's pow decide otherwise); a row with flag 0 is scikit-learn's answer, indices and distance bits.  1 <= n <= 2^30,
+ * n_nodes = 2^L - 1 with 2^(L-1) <= n, 1 <= k <= min(n, 63). */
+int tgn_kdtree_query(int n, int n_nodes, int k, const double *xyz, const long long *idx_array, const long long *node_data,
+                     const double *node_bounds, int m, const double *queries, const long long *rows, int n_rows, long long *idx,
+                     double *dist, unsigned char *flag, void *stream);
+
 /* Exact float64 kNN with a fused label vote: the answer of sklearn KDTree(xyz).query(queries, k) -- boundary detection of
  * InferencePipeLine.get_boundary_sampled_feats (inference_pipeline_tgn.py:289-330).  xyz (n,3) and queries (m,3) float64
  * DEVICE; 1 <= k <= 64, k <= n.  Distances d2 = (dx*dx + dy*dy) + dz*dz in float64 without contraction, neighbours ascending

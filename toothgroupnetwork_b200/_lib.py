@@ -62,6 +62,7 @@ _SIGS = {
     "tgn_kmeans": [_i, ctypes.c_longlong, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_meanshift": [_i, _i, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _i, _vp, _vp, _vp],
     "tgn_kdtree_build": [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp],
+    "tgn_kdtree_query": [_i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp],
 }
 
 

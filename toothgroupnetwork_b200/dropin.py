@@ -98,20 +98,22 @@ def accelerate_inference_pipeline(module=None) -> None:
     boundary.accelerate(module)
 
 
-def accelerate_label_transfer(module=None) -> None:
+def accelerate_label_transfer(module=None, ties: str = "host") -> None:
     """Optional: answer the float64 ``KDTree.query`` calls of the inference pipelines' label transfers on the GPU through
     ``toothgroupnetwork_b200.neighbors.KDTree`` (the boundary clusters and the final transfer to the mesh,
     inference_pipeline_tgn.py:107-114, :137-140; the final transfers of inference_pipeline_tsegnet.py:72-74 and
-    inference_pipeline_sem.py:37-39), with the same indices and distances.  Swaps the ``KDTree`` name of
+    inference_pipeline_sem.py:37-39), with the same indices and distances.  Rows with exactly tied distances are answered by
+    scikit-learn's query code on a device-built tree (ties="host"), or by the same depth-first walk on the device
+    (ties="device": ``neighbors.DeviceKDTree``, only the rows the walk flags reach the host).  Swaps the ``KDTree`` name of
     ``inference_pipelines.inference_pipeline_tgn`` (imported from ``sys.path`` when no module is passed), and of the tsegnet and
     sem pipelines when they are already imported.  ``ops_utils`` keeps its own: ``accelerate_ops_utils`` replaces its queries."""
     from . import neighbors
     if module is None:
         module = importlib.import_module("inference_pipelines.inference_pipeline_tgn")
-    neighbors.accelerate(module)
+    neighbors.accelerate(module, ties)
     for name in ("inference_pipelines.inference_pipeline_tsegnet", "inference_pipelines.inference_pipeline_sem"):
         if name in sys.modules:
-            neighbors.accelerate(sys.modules[name])
+            neighbors.accelerate(sys.modules[name], ties)
 
 
 def accelerate_dgcnn(module=None) -> None:

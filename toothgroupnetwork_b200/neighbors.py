@@ -15,7 +15,11 @@ The tree those rows need is scikit-learn's, bit for bit, and ``sklearn_tree`` bu
 DESIGN §3.16): on the first flagged row its arrays are copied to the host once and a scikit-learn ``KDTree`` is restored from
 them with ``__setstate__``, without a host build.  An installation whose pickled state has another layout builds it on the host.
 
-``accelerate(module)`` points a module's ``KDTree`` name at the class.  scikit-learn is imported only when a row is flagged.
+``DeviceKDTree`` answers the flagged rows on the device instead: ``sklearn_query`` walks that tree the way scikit-learn's
+``query`` does (csrc/kdtree_query.cu, DESIGN §3.17), and only the rows whose walk it flags reach scikit-learn's query code.
+
+``accelerate(module, ties)`` points a module's ``KDTree`` name at one of the classes.  scikit-learn is imported only when a row
+is flagged.
 """
 from __future__ import annotations
 
@@ -120,8 +124,12 @@ class KDTree:
         out = torch.empty(n_idx + n_dist + m, dtype=torch.uint8, device=self.device)
         idx = out[:n_idx].view(torch.int64).view(m, k)
         dist = out[n_idx:n_idx + n_dist].view(torch.float64).view(m, k) if return_distance else None
-        self._launch(torch.from_numpy(X).to(self.device), k, idx, dist, out[n_idx + n_dist:])
+        queries = torch.from_numpy(X).to(self.device)
+        self._launch(queries, k, idx, dist, out[n_idx + n_dist:])
         host = out.cpu().numpy()
+        tied = np.flatnonzero(host[n_idx + n_dist:])
+        if tied.size:
+            host = self._walk_ties(queries, k, idx, dist, out[n_idx + n_dist:], tied, out, host)
         ind = host[:n_idx].view(np.intp).reshape(m, k)
         d = host[n_idx:n_idx + n_dist].view(np.float64).reshape(m, k) if return_distance else None
         rows = np.flatnonzero(host[n_idx + n_dist:])
@@ -134,6 +142,40 @@ class KDTree:
             else:
                 ind[rows] = self._host_tree.query(X[rows], k=k, return_distance=False)
         return (d, ind) if return_distance else ind
+
+    def _walk_ties(self, queries, k, idx, dist, flag, tied, out, host):
+        """The rows the grid flags (``tied``, ascending) before the host fallback: here all of them stay flagged.  Returns the
+        host copy of ``out``, whose flag bytes name the rows left to the host."""
+        return host
+
+
+class DeviceKDTree(KDTree):
+    """``KDTree`` whose tied rows are answered on the device: scikit-learn's own depth-first walk over its own tree
+    (``sklearn_query`` on ``sklearn_tree(X, leaf_size, radius=False)``, built once on the first tie, nothing copied to the
+    host).  Only the rows the walk flags go to scikit-learn's query code (``host_rows``); ``walk_rows`` counts the rows the walk
+    answered.  A tree outside the device build's range, a leaf_size that is not an integer or a scikit-learn whose pickled
+    KDTree has another layout than the 1.9 the walk restates keep every tied row on the host, as ``KDTree`` does."""
+
+    def __init__(self, X, leaf_size: int = 40, metric: str = "minkowski", **kwargs):
+        super().__init__(X, leaf_size, metric, **kwargs)
+        self.walk_rows = 0
+        self._walk_tree = None
+        self._walk_ok = None
+
+    def _walk_ties(self, queries, k, idx, dist, flag, tied, out, host):
+        if self._walk_ok is None:
+            ls = self.leaf_size
+            self._walk_ok = (not isinstance(ls, bool) and isinstance(ls, (int, np.integer))
+                             and int(L.load().tgn_kdtree_nodes(self._n, int(ls))) == tree_nodes(self._n, int(ls))
+                             and _sklearn_layout_ok())
+        if not self._walk_ok:
+            return host
+        if self._walk_tree is None:
+            self._walk_tree = sklearn_tree(self._xyz, int(self.leaf_size), radius=False)
+        _walk(self._walk_tree, queries, k, torch.from_numpy(tied).to(self.device), idx, dist, flag)
+        host = out.cpu().numpy()
+        self.walk_rows += int(tied.size) - int(np.count_nonzero(host[host.size - flag.numel():]))
+        return host
 
 
 NODE_DATA = np.dtype([("idx_start", "<i8"), ("idx_end", "<i8"), ("is_leaf", "<i8"), ("radius", "<f8")])   # NodeData_t
@@ -209,6 +251,71 @@ def sklearn_tree(X, leaf_size: int = 40, radius: bool = True):
     return xyz, idx, node_data, bounds
 
 
+def _walk(tree, queries: torch.Tensor, k: int, rows, idx, dist, flag) -> None:
+    """csrc/kdtree_query.cu on the current stream: rows (int64 on the device) or every row when None"""
+    xyz, idx_array, node_data, bounds = tree
+    L.call("tgn_kdtree_query", int(xyz.shape[0]), int(node_data.shape[0]), int(k), L.ptr(xyz), L.ptr(idx_array),
+           L.ptr(node_data), L.ptr(bounds), int(queries.shape[0]), L.ptr(queries), L.ptr(rows),
+           0 if rows is None else int(rows.numel()), L.ptr(idx), L.ptr(dist), L.ptr(flag), L.stream_ptr())
+
+
+def sklearn_query(tree, queries: torch.Tensor, k: int = 1, rows=None):
+    """``sklearn.neighbors.KDTree(X, leaf_size).query(queries, k)`` walked on the GPU over ``tree``, the tuple
+    ``sklearn_tree(X, leaf_size, radius=False)`` returns: scikit-learn's depth-first visit order, its heap and its final sort
+    (csrc/kdtree_query.cu, DESIGN §3.17).  queries (m, 3) float64 CUDA -> (dist float64 (m, k), idx int64 (m, k),
+    flag uint8 (m)) on the device.  Every row with flag 0 is scikit-learn's answer, indices and distance bits; a flagged row
+    compared a node bound within 2^-40 of the other operand where scikit-learn's ``pow`` could round differently.
+    ``rows`` (row numbers, host or device) restricts the walk to those rows; the other rows of the outputs are left
+    uninitialised.  Refusals raise before any launch: scikit-learn's ValueError where it refuses (empty or non-finite
+    queries, another width, k > n), TgnError for what is not implemented (k outside 1..63, non-CUDA or non-float64 queries, a
+    malformed tree)."""
+    if not isinstance(tree, tuple) or len(tree) != 4 or not all(torch.is_tensor(t) for t in tree):
+        raise L.TgnError("sklearn_query: tree must be the tuple sklearn_tree(X, leaf_size, radius=False) returns")
+    xyz, idx_array, node_data, bounds = tree
+    L.require_cuda(*tree)
+    n, n_nodes = int(xyz.shape[0]), int(node_data.shape[0])
+    if (xyz.dtype != torch.float64 or idx_array.dtype != torch.int64 or node_data.dtype != torch.int64
+            or bounds.dtype != torch.float64 or tuple(xyz.shape) != (n, 3) or tuple(idx_array.shape) != (n,)
+            or tuple(node_data.shape) != (n_nodes, 4) or tuple(bounds.shape) != (2, n_nodes, 3)
+            or not all(t.is_contiguous() and t.device == xyz.device for t in tree)
+            or not 1 <= n <= 2 ** 30 or n_nodes & (n_nodes + 1) or (n_nodes + 1) // 2 > n):
+        raise L.TgnError("sklearn_query: tree must be the tuple sklearn_tree(X, leaf_size, radius=False) returns")
+    if not torch.is_tensor(queries) or queries.dtype != torch.float64:
+        raise L.TgnError(f"sklearn_query: queries must be a float64 CUDA tensor, got "
+                         f"{queries.dtype if torch.is_tensor(queries) else type(queries)}")
+    L.require_cuda(queries)
+    if queries.device != xyz.device:
+        raise L.TgnError(f"sklearn_query: queries on {queries.device}, tree on {xyz.device}")
+    if queries.dim() != 2:
+        raise ValueError(f"Expected 2D array, got {queries.dim()}D array instead")
+    if queries.shape[0] == 0:
+        raise ValueError(f"Found array with 0 sample(s) (shape={tuple(queries.shape)}) while a minimum of 1 is required.")
+    if queries.shape[1] != 3:
+        raise ValueError("query data dimension must match training data dimension")
+    if not bool(torch.isfinite(queries).all()):
+        raise ValueError("Input contains NaN or infinity.")
+    k = operator.index(k)
+    if n < k:
+        raise ValueError("k must be less than or equal to the number of training points")
+    if not 1 <= k <= MAX_K:
+        raise L.TgnError(f"sklearn_query: need 1 <= k <= {MAX_K}, got k={k}")
+    m = int(queries.shape[0])
+    if rows is not None:
+        host_rows = np.asarray(rows.cpu() if torch.is_tensor(rows) else rows)
+        if host_rows.ndim != 1 or (host_rows.size and host_rows.dtype.kind not in "iu"):
+            raise L.TgnError("sklearn_query: rows must be a 1-D array of row numbers")
+        if host_rows.size and (host_rows.min() < 0 or host_rows.max() >= m):
+            raise L.TgnError(f"sklearn_query: rows must lie in [0, {m})")
+        rows = torch.from_numpy(host_rows.astype(np.int64)).to(xyz.device)
+    queries = queries.contiguous()
+    idx = torch.empty((m, k), dtype=torch.int64, device=xyz.device)
+    dist = torch.empty((m, k), dtype=torch.float64, device=xyz.device)
+    flag = torch.empty(m, dtype=torch.uint8, device=xyz.device)
+    if rows is None or rows.numel():
+        _walk(tree, queries, k, rows, idx, dist, flag)
+    return dist, idx, flag
+
+
 def host_kdtree_class():
     """The host class the tie fallback restores (or, on an unexpected state layout, builds): scikit-learn's KDTree."""
     from sklearn.neighbors import KDTree as HostKDTree
@@ -232,6 +339,13 @@ def _state_layout_ok(cls) -> bool:
         except Exception:
             _state_ok = False
     return _state_ok
+
+
+def _sklearn_layout_ok() -> bool:
+    """Whether the installed scikit-learn is the 1.9 whose query the device walk restates, judged by its KDTree's state
+    layout (the check the tie fallback's restore makes, shared with it)."""
+    from sklearn.neighbors import KDTree as SkKDTree
+    return _state_layout_ok(SkKDTree)
 
 
 def host_tree(X: np.ndarray, xyz: torch.Tensor, leaf_size: int):
@@ -261,8 +375,12 @@ def restore(cls, X: np.ndarray, idx_array: np.ndarray, node_data: np.ndarray, no
     return tree
 
 
-def accelerate(module) -> None:
+def accelerate(module, ties: str = "host") -> None:
     """Point a module's ``KDTree`` name (``from sklearn.neighbors import KDTree`` in inference_pipeline_tgn.py:6,
-    inference_pipeline_tsegnet.py:5, inference_pipeline_sem.py:4) at the device implementation."""
+    inference_pipeline_tsegnet.py:5, inference_pipeline_sem.py:4) at the device implementation: ``KDTree`` with
+    ties="host", ``DeviceKDTree`` (tied rows walked on the device) with ties="device"."""
+    classes = {"host": KDTree, "device": DeviceKDTree}
+    if ties not in classes:
+        raise ValueError(f"ties must be 'host' or 'device', got {ties!r}")
     if hasattr(module, "KDTree"):
-        module.KDTree = KDTree
+        module.KDTree = classes[ties]
