@@ -3,11 +3,14 @@ bitwise against the CPU oracle, int64 and int32 outputs.  The cases aim at the w
 the window size or smaller than one window, balls whose members are spread over several windows (full in a later one, or
 never full), K from 1 to 128, duplicated vertices, clouds far from the origin, and clouds whose window grows to keep the
 (window, cell) table within bounds."""
+import ctypes
+
 import numpy as np
 import pytest
 import torch
 
 from oracle import oracle
+from toothgroupnetwork_b200 import _lib as L
 from toothgroupnetwork_b200 import clouds
 from toothgroupnetwork_b200 import pointnet2_utils as pn2
 
@@ -74,6 +77,100 @@ CASES = [
 def test_windowed_grid_matches_oracle(N, S, r, K, offset, scale, dup):
     xyz, new = arch_batch(N, S, r, offset, scale, dup=dup)
     check_all_paths(xyz, new, r, K)
+
+
+def ball_float64(xyz, new, r, K):
+    """query_ball_point in float64, exact on the 1/8 lattice (tests/test_cpu_lattice_exact.py): the first K indices with
+    d2 <= r^2, padded with the first, N for an empty ball; and how many (query, point) pairs lie exactly on a sphere."""
+    x, q = xyz.double().numpy(), new.double().numpy()
+    B, N, _ = x.shape
+    out = np.full((B, q.shape[1], K), N, np.int64)
+    on_sphere = 0
+    for b in range(B):
+        for c in range(0, q.shape[1], 128):
+            d = q[b, c:c + 128, None, :] - x[b][None, :, :]
+            d2 = (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2]
+            on_sphere += int((d2 == r * r).sum())
+            for s, inside in enumerate(d2 <= r * r):
+                m = np.nonzero(inside)[0][:K]
+                if len(m):
+                    out[b, c + s, :] = m[0]
+                    out[b, c + s, :len(m)] = m
+    return out, on_sphere
+
+
+def lattice_batch(half, N, S, seed, B=2):
+    """B shuffled 1/8 lattices (N points of the box |i| <= half each) and S queries per cloud: a quarter on points of the
+    cloud, a quarter on lattice sites the cloud may lack, a quarter in the middle of cells, the rest half-way along a cell edge."""
+    g = torch.Generator().manual_seed(seed)
+    xs = [clouds.lattice(half, seed + b, N) for b in range(B)]
+    news = []
+    for x in xs:
+        q = S // 4
+        on = x[torch.randperm(N, generator=g)[:q]]
+        site = torch.randint(-half, half + 1, (q, 3), generator=g).float() / 8.0
+        mid = (2 * torch.randint(-half, half, (q, 3), generator=g) + 1).float() / 16.0
+        edge = torch.randint(-half, half, (S - 3 * q, 3), generator=g).float() / 8.0
+        edge[:, 0] += 1.0 / 16.0
+        news.append(torch.cat([on, site, mid, edge]))
+    return torch.stack(xs).contiguous(), torch.stack(news).contiguous()
+
+
+LATTICE_CASES = [
+    # (half-width of the lattice box, points per cloud, queries, r, K): r = 0.25 puts 6 lattice points of a full shell at
+    # exactly r (d2 = float32(r^2) = 1/16) and 33 in a ball around a lattice point, 32 around a cell centre
+    (10, 9261, 512, 0.25, 32),           # every point of the box: full balls, K one below the 33 members
+    (10, 9261, 512, 0.25, 33),           # K = the members of an interior ball
+    (10, 9261, 512, 0.25, 34),           # K one above: padded with the first
+    (10, 9261, 256, 0.25, 1),
+    (10, 9261, 256, 0.375, 128),         # 123 / 136 members at r = 3/8 (shell i^2 + j^2 + l^2 = 9 at exactly r)
+    (40, 24000, 1024, 0.25, 8),          # 4.5 % of a larger box: sparse balls, the grid's case
+    (40, 24000, 1024, 0.5, 16),          # ~12 members: 4.5 % of the 257 sites within r = 0.5
+    (6, 2197, 300, 0.25, 32),            # below the grid's automatic size: the tile kernel, and the grid when forced
+]
+
+
+@pytest.mark.parametrize("half,N,S,r,K", LATTICE_CASES)
+def test_lattice_balls_match_oracle_and_float64(half, N, S, r, K):
+    xyz, new = lattice_batch(half, N, S, seed=half + N + K)
+    want = check_all_paths(xyz, new, r, K)
+    exact, on_sphere = ball_float64(xyz, new, r, K)
+    assert np.array_equal(want, exact)
+    assert on_sphere > 0, "no point exactly on a sphere"
+
+
+SENTINEL = -0x21524111                 # never an index: shows a row that neither kernel wrote
+
+
+@pytest.mark.parametrize("wide", [False, True])
+def test_one_launch_mixing_grid_and_tile_clouds(wide):
+    """Three clouds of one launch: two sparse ones the automatic choice sends to the grid kernel, and a copy of the arch
+    shrunk until r covers it whole, left to the tile kernel (every point a member).  The per-cloud flag decides which kernel
+    writes which rows, so into a sentinel-filled output every row must be written once, by either.  wide: enough queries
+    that the tile kernel runs at 16 warps per CTA."""
+    N, r, K = 24000, 0.1, 32
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    S = 16 * -(-2 * sms // 3) if wide else 256
+    assert (3 * -(-S // 16) >= 2 * sms) == wide
+    arch = clouds.dental_arch(N, 21)[0]
+    dense = (arch - arch.mean(0)) * 0.02                               # extent ~0.03 < r
+    sparse = clouds.lattice(40, 22, N)
+    assert float((dense.max(0).values - dense.min(0).values).norm()) < r
+    xyz = torch.stack([arch, dense, sparse]).contiguous()
+    g = torch.Generator().manual_seed(23)
+    new = torch.stack([c[torch.randperm(N, generator=g)[:S]] for c in xyz]).contiguous()
+    new[2, : S // 2] += 1.0 / 16.0                                     # off-lattice queries: empty balls
+    want = oracle.query_ball_point(r, K, xyz.numpy(), new.numpy())
+    assert (want[1] == np.arange(K)).all()                            # the dense cloud: every ball holds the first K points
+    x, q = xyz.cuda(), new.cuda()
+    for idx64, dtype in ((1, torch.int64), (0, torch.int32)):
+        for path in (pn2.BALL_AUTO, pn2.BALL_GRID, pn2.BALL_TILE):
+            out = torch.full((3, S, K), SENTINEL, dtype=dtype, device="cuda")
+            L.call("tgn_ball_query", 3, N, S, ctypes.c_float(pn2._radius_sq_f32(r)), K, L.ptr(x), L.ptr(q), L.ptr(out),
+                   idx64 | path, L.stream_ptr())
+            got = out.cpu().numpy().astype(np.int64)
+            assert np.array_equal(got, want), f"path {path}, idx64 {idx64}: rows differ in clouds " \
+                                              f"{sorted(set(np.nonzero((got != want).any(-1))[0].tolist()))}"
 
 
 def planted_cloud(N, member_idx, seed):

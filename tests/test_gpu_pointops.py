@@ -123,6 +123,34 @@ def test_fps_full_size_properties():
 
 
 # ------------------------------------------------------------------------------------ kNN
+REF_MAX_K = 100                 # the reference kernel's heap holds 100 entries (best_dist[100]): larger k is not asked of it
+
+
+def cell_centres(half, n, seed):
+    """n points in the middle of cells of the 1/8 lattice |i| <= half: their 8 nearest lattice points tie"""
+    g = torch.Generator().manual_seed(seed)
+    return ((2 * torch.randint(-half, half, (n, 3), generator=g) + 1).float() / 16.0).contiguous()
+
+
+def lattice_with_centres(half, n, seed):
+    """a shuffled 1/8 lattice with n cell centres among its points: self-queries at the centres tie 8 ways at rank 1"""
+    x = torch.cat([clouds.lattice(half, seed), cell_centres(half, n, seed)])
+    return x[torch.randperm(x.shape[0], generator=torch.Generator().manual_seed(seed))].contiguous()
+
+
+def float64_k_smallest(xyz, q, off, noff, k):
+    """per query, the k smallest float64 squared distances to the points of its segment, ascending, padded with 1e10 as the
+    kernels pad segments shorter than k: exactly the kernels' float32 d2 on lattice inputs (tests/test_cpu_lattice_exact.py)"""
+    x, qq = xyz.double().numpy(), q.double().numpy()
+    out = np.full((qq.shape[0], k), float(np.float32(1e10)))
+    for s, e, qs, qe in zip([0] + list(off[:-1]), off, [0] + list(noff[:-1]), noff):
+        for c in range(qs, qe, 256):
+            d = qq[c:min(c + 256, qe), None, :] - x[None, s:e, :]
+            d2 = np.sort((d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1]) + d[..., 2] * d[..., 2], axis=1)
+            out[c:c + d2.shape[0], :min(k, e - s)] = d2[:, :k]
+    return out
+
+
 KNN_CASES = [
     ("self_k16", lambda: clouds.cube(4096, 1), None, [4096], None, 16),
     ("self_k36", lambda: clouds.dental_arch(6000, 2)[0], None, [6000], None, 36),
@@ -133,6 +161,14 @@ KNN_CASES = [
     ("k1", lambda: clouds.cube(2000, 7), 500, [2000], [500], 1),
     ("k64", lambda: clouds.cube(1000, 8), None, [1000], None, 64),
     ("k100", lambda: clouds.cube(700, 9), None, [700], None, 100),
+    # 1/8 lattices below the grid's size (KNN_GRID_MIN_POINTS): whole shells tie, d2 exact
+    ("lattice1331_self_k1", lambda: clouds.lattice(5, 1), None, [1331], None, 1),
+    ("lattice1331_self_k3", lambda: clouds.lattice(5, 2), None, [1331], None, 3),
+    ("lattice_and_cell_centres_k36", lambda: lattice_with_centres(5, 300, 3), None, [1631], None, 36),
+    ("lattice_and_cell_centres_k126", lambda: lattice_with_centres(5, 300, 4), None, [1631], None, 126),
+    ("lattice_and_cell_centres_k127", lambda: lattice_with_centres(5, 300, 5), None, [1631], None, 127),
+    ("lattice_segments_shorter_than_k127", lambda: torch.cat([clouds.lattice(3, 6, 60), clouds.lattice(5, 7), clouds.lattice(1, 8)]),
+     700, [60, 1391, 1418], [20, 680, 700], 127),
 ]
 
 
@@ -158,11 +194,15 @@ def test_knn_matches_oracle(name, build, m, off, noff, k):
     idx2, dist = pointops.knnquery(k, xyz.cuda(), new_xyz.cuda(), i32(off), i32(noff))
     assert torch.equal(idx2, idx)
     assert np.array_equal(dist.cpu().numpy().view(np.uint32), w_dist.view(np.uint32))
+    if name.startswith("lattice"):
+        assert np.array_equal(d2.cpu().numpy().astype(np.float64), float64_k_smallest(xyz, new_xyz, off, noff, k))
 
 
 @needs_ref
 @pytest.mark.parametrize("name,build,m,off,noff,k", KNN_CASES, ids=[c[0] for c in KNN_CASES])
 def test_knn_matches_reference_kernel(name, build, m, off, noff, k):
+    if k > REF_MAX_K:
+        pytest.skip(f"the reference kernel holds at most {REF_MAX_K} neighbours")
     xyz, new_xyz, off, noff = _knn_inputs(build, m, off, noff)
     x, q, o, no = xyz.cuda(), new_xyz.cuda(), i32(off), i32(noff)
     r_idx, r_d2 = ref_cuda.knnquery(k, x, q, o, no)
@@ -188,6 +228,16 @@ GRID_CASES = [
     ("flat_cloud_k16", lambda: clouds.cube(6000, 9) * torch.tensor([1.0, 1.0, 0.0]), [6000], None, None, 16),
     ("all_points_equal_k8", lambda: torch.ones(3000, 3), [3000], None, None, 8),
     ("k100", lambda: clouds.dental_arch(9000, 11)[0], [9000], None, None, 100),
+    # 1/8 lattices above KNN_GRID_MIN_POINTS: whole shells tie (the heap emulation), d2 exact; queries in the middle of cells
+    # tie 8 ways at rank 1
+    ("lattice9261_self_k36", lambda: clouds.lattice(10, 12), [9261], None, None, 36),
+    ("lattice_cell_centres_k1", lambda: clouds.lattice(8, 13), [4913], lambda x: cell_centres(8, 3000, 13), [3000], 1),
+    ("lattice_cell_centres_k3", lambda: clouds.lattice(8, 14), [4913], lambda x: cell_centres(8, 3000, 14), [3000], 3),
+    ("lattice_cell_centres_k100", lambda: clouds.lattice(8, 15), [4913], lambda x: cell_centres(8, 2000, 15), [2000], 100),
+    ("lattice_cell_centres_k126", lambda: clouds.lattice(8, 16), [4913], lambda x: cell_centres(8, 2000, 16), [2000], 126),
+    ("lattice_cell_centres_k127", lambda: clouds.lattice(8, 17), [4913], lambda x: cell_centres(8, 2000, 17), [2000], 127),
+    ("lattice_segments_shorter_than_k127", lambda: torch.cat([clouds.lattice(3, 18, 60), clouds.lattice(8, 19), clouds.lattice(1, 20),
+                                                               clouds.lattice(6, 21, 2000)]), list(np.cumsum([60, 4913, 27, 2000])), None, None, 127),
 ]
 
 
@@ -214,17 +264,36 @@ def test_knn_grid_equals_bruteforce_kernel_and_reference(name, build, off, qbuil
     c_idx, c_d2 = pointops.knn_packed(k, x, qq, o, no)           # identical repeated query: served from the cache
     assert L.launch_count() == launches and c_idx is g_idx
     k2 = k // 2 if k > 1 else 2
-    h_idx, _ = pointops.knn_packed(k2, x, qq, o, no)             # same grid, other k: one launch
+    h_idx, h_d2 = pointops.knn_packed(k2, x, qq, o, no)          # same grid, other k: one launch
     assert L.launch_count() - launches == 1
     kk = min(k, k2)
-    assert torch.equal(h_idx[:, :kk], b_idx[:, :kk]) or name.startswith(("duplicated", "all_points"))
-    if ref_cuda.available():
+    assert torch.equal(h_idx[:, :kk], b_idx[:, :kk]) or name.startswith(("duplicated", "all_points", "lattice"))
+    assert torch.equal(h_d2[:, :kk].view(torch.int32), b_d2[:, :kk].view(torch.int32))
+    w_idx, _, w_d2 = oracle.knnquery(k, xyz.numpy(), q.numpy(), np.asarray(off, np.int32), np.asarray(off if noff is None else noff, np.int32))
+    assert np.array_equal(g_idx.cpu().numpy(), w_idx) and np.array_equal(g_d2.cpu().numpy().view(np.uint32), w_d2.view(np.uint32))
+    if name.startswith("lattice"):
+        want = float64_k_smallest(xyz, q, np.asarray(off), np.asarray(off if noff is None else noff), k)
+        assert np.array_equal(g_d2.cpu().numpy().astype(np.float64), want)
+    if ref_cuda.available() and k <= REF_MAX_K:
         r_idx, r_d2 = ref_cuda.knnquery(k, x, qq, o, no)
         assert torch.equal(g_d2.view(torch.int32), r_d2.view(torch.int32)) and torch.equal(g_idx, r_idx)
     x.add_(0.0)                                                   # in-place write bumps the version: caches must miss
     launches = L.launch_count()
     pointops.knn_packed(k, x, qq if qbuild is not None else x, o, no)
     assert L.launch_count() - launches == 5
+
+
+@pytest.mark.parametrize("grid", [False, True])
+def test_knn_refuses_k_above_127(grid):
+    xyz = clouds.lattice(8, 22).cuda()
+    o = i32([4913])
+    pointops.clear_knn_caches()
+    pointops.set_knn_grid(grid)
+    try:
+        with pytest.raises(L.TgnError, match="nsample=128 exceeds 127"):
+            pointops.knn_packed(128, xyz, xyz, o, o)
+    finally:
+        pointops.set_knn_grid(True)
 
 
 def test_knn_full_size_property():

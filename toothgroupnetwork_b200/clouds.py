@@ -66,6 +66,23 @@ def boundary_inputs(m: int, seed: int = 0, n_sampled: int = 24000, label_noise: 
     return org, org[rows].copy(), labels
 
 
+LATTICE_STEP = 0.125
+LATTICE_HALF = 64
+
+
+def lattice(half: int, seed: int = 0, n: int | None = None) -> torch.Tensor:
+    """The points (i, j, l) / 8 with |i|, |j|, |l| <= half (half <= LATTICE_HALF), shuffled by the seed; the first n of them when
+    n is given.  On these coordinates, and on queries on the half-step lattice (2i + 1) / 16 between them, every product and
+    partial sum of the float32 distance forms the kernels evaluate is exact, so their distances equal float64's and tie
+    wherever the true distances do (tests/test_cpu_lattice_exact.py): the tie stress input of the neighbour selections."""
+    assert 0 <= half <= LATTICE_HALF
+    g = torch.Generator().manual_seed(int(seed) + 104723)
+    axis = torch.arange(-half, half + 1, dtype=torch.float32) * LATTICE_STEP
+    pts = torch.cartesian_prod(axis, axis, axis)
+    pts = pts[torch.randperm(pts.shape[0], generator=g)]
+    return (pts if n is None else pts[:n]).contiguous()
+
+
 def with_duplicates(xyz: torch.Tensor, seed: int = 0) -> torch.Tensor:
     """Every vertex twice, shuffled: the FPS / kNN tie-break stress input (SURVEY.md 7.1)."""
     g = torch.Generator().manual_seed(int(seed) + 7919)

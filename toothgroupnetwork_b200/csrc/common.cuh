@@ -14,7 +14,7 @@ namespace tgn {
 void set_error(const char* fmt, ...);
 int check_launch(const char* what);   // cudaGetLastError -> status (+ message)
 int sm_count();                       // of the current device (cached per device)
-int ensure_dynamic_smem(const void* func, size_t bytes);   // per (device, kernel) opt-in to > 48 KB of dynamic shared memory
+int ensure_dynamic_smem(const void* func, size_t bytes);   // per (device, kernel) opt-in to > 48 KB of static + dynamic shared memory
 void keep_async_pool();               // configure the default cudaMallocAsync pool to cache freed scratch
 
 // ---------------------------------------------------------------- fp32 pairs

@@ -11,8 +11,9 @@
 //      significant first; every pass re-evaluates the distances (24 000 points / 1024 threads: ~24 each) and histograms the
 //      digit of the keys that still match the prefix in shared memory;
 //   2. COMPACTION of the k selected (key, index) pairs into shared memory: everything below the threshold, plus as many
-//      threshold-equal points as are needed, lowest index first (the equal-key candidates are collected and rank-sorted,
-//      so the choice does not depend on scheduling);
+//      threshold-equal points as are needed, lowest index first: when more points tie at the threshold than are taken,
+//      sweeps over ascending blocks of 1024 indices rank the equal keys with a block scan, so however many tie, the choice
+//      does not depend on scheduling;
 //   3. BITONIC SORT of the k pairs (padded to a power of two) by (distance, index), written out in ascending order -- the
 //      order KDTree.query(sort_results=True) returns and the second-stage network depends on (its FPS starts at crop row 0).
 // Distances are evaluated in float64 on the float32 coordinates, ((dx*dx + dy*dy) + dz*dz) unfused, like sklearn's
@@ -27,6 +28,7 @@ namespace {
 
 constexpr int kT = 1024;
 constexpr int kMaxK = 4096;
+static_assert(kT == 32 * 32, "the compaction's block scan takes one warp total per lane");
 
 __device__ __forceinline__ unsigned long long dist_key(const float* __restrict__ p, double qx, double qy, double qz) {
     const double dx = static_cast<double>(__ldg(p)) - qx, dy = static_cast<double>(__ldg(p + 1)) - qy, dz = static_cast<double>(__ldg(p + 2)) - qz;
@@ -41,8 +43,8 @@ __global__ void __launch_bounds__(kT) crop_knn_kernel(int N, int Q, int k, int k
     extern __shared__ __align__(16) unsigned char dyn[];
     unsigned long long* skey = reinterpret_cast<unsigned long long*>(dyn);            // [kpad]
     int* sidx = reinterpret_cast<int*>(skey + kpad);                                  // [kpad]
-    int* seq = sidx + kpad;                                                           // [kpad] threshold-equal candidates
     __shared__ unsigned hist[256];
+    __shared__ unsigned s_wcnt[2][kT / 32];                                           // threshold-equal keys per warp
     __shared__ unsigned long long s_prefix;
     __shared__ int s_need, s_count, s_eq;
 
@@ -53,8 +55,9 @@ __global__ void __launch_bounds__(kT) crop_knn_kernel(int N, int Q, int k, int k
     const double qx = static_cast<double>(__ldg(c)), qy = static_cast<double>(__ldg(c + 1)), qz = static_cast<double>(__ldg(c + 2));
     const int kk = min(k, N);
 
-    // ---- 1. radix select: after the loop s_prefix is the kk-th smallest key, s_need how many keys EQUAL to it are taken ----
-    if (tid == 0) { s_prefix = 0ull; s_need = kk; }
+    // ---- 1. radix select: after the loop s_prefix is the kk-th smallest key, s_need how many keys EQUAL to it are taken and
+    //         s_eq how many there are ----
+    if (tid == 0) { s_prefix = 0ull; s_need = kk; s_count = 0; }
     __syncthreads();
     for (int pass = 0; pass < 8; ++pass) {
         const int shift = 56 - 8 * pass;
@@ -76,37 +79,50 @@ __global__ void __launch_bounds__(kT) crop_knn_kernel(int N, int Q, int k, int k
             }
             s_prefix = prefix | (static_cast<unsigned long long>(d) << shift);
             s_need = need;                                   // still to be found inside digit d
+            s_eq = static_cast<int>(hist[d]);                // keys inside digit d; after the last pass, keys == the kk-th
         }
         __syncthreads();
     }
     const unsigned long long thr = s_prefix;
     const int need_eq = s_need;                              // number of keys == thr that belong to the answer
+    const bool all_eq = s_eq == need_eq;                     // all of them: nothing to choose
 
     // ---- 2. compaction ----------------------------------------------------------------------------------------------
-    if (tid == 0) { s_count = 0; s_eq = 0; }
-    __syncthreads();
+    // The kk - need_eq keys below thr, and the threshold-equal keys when all of them are taken, go to [0, kk) in arrival
+    // order (the sort orders them).
     for (int j = tid; j < N; j += kT) {
         const unsigned long long key = dist_key(pts + 3 * static_cast<size_t>(j), qx, qy, qz);
-        if (key < thr) {
+        if (key < thr || (all_eq && key == thr)) {
             const int pos = atomicAdd(&s_count, 1);
             skey[pos] = key; sidx[pos] = j;
-        } else if (key == thr) {
-            const int pos = atomicAdd(&s_eq, 1);
-            if (pos < kpad) seq[pos] = j;                    // more than kpad exact ties cannot all be needed
         }
     }
-    __syncthreads();
-    {
-        const int below = s_count, neq = min(s_eq, kpad);
-        // the need_eq lowest indices among the threshold-equal points (rank by index: scheduling-independent)
-        for (int i = tid; i < neq; i += kT) {
-            const int v = seq[i];
-            int rank = 0;
-            for (int j = 0; j < neq; ++j) rank += seq[j] < v ? 1 : 0;
-            if (rank < need_eq) { skey[below + rank] = thr; sidx[below + rank] = v; }
+    // More keys equal thr than are taken: the need_eq of lowest index go to [kk - need_eq, kk).  Each sweep covers kT
+    // consecutive indices, one per thread, and a block scan (a ballot per warp, then the warp totals) gives every equal key
+    // the number of equal keys at lower indices; the sweeps stop once need_eq are placed.
+    if (!all_eq) {
+        const int lane = tid & 31, warp = tid >> 5;
+        int taken = 0;                                       // equal keys at lower indices than this sweep (block-uniform)
+        for (int base = 0, sweep = 0; base < N && taken < need_eq; base += kT, ++sweep) {
+            const int j = base + tid;
+            const bool eq = j < N && dist_key(pts + 3 * static_cast<size_t>(j), qx, qy, qz) == thr;
+            const unsigned m = __ballot_sync(0xffffffffu, eq);
+            unsigned* wcnt = s_wcnt[sweep & 1];              // alternate: the previous sweep's totals may still be read
+            if (lane == 0) wcnt[warp] = __popc(m);
+            __syncthreads();
+            const unsigned c = wcnt[lane];                   // one warp total per lane (kT / 32 == 32 warps)
+            unsigned incl = c;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            const int rank = taken + static_cast<int>(__shfl_sync(0xffffffffu, incl - c, warp)) + __popc(m & ((1u << lane) - 1u));
+            if (eq && rank < need_eq) { skey[kk - need_eq + rank] = thr; sidx[kk - need_eq + rank] = j; }
+            taken += static_cast<int>(__shfl_sync(0xffffffffu, incl, 31));
         }
-        for (int i = below + need_eq + tid; i < kpad; i += kT) { skey[i] = ~0ull; sidx[i] = INT_MAX; }      // padding sorts last
     }
+    for (int i = kk + tid; i < kpad; i += kT) { skey[i] = ~0ull; sidx[i] = INT_MAX; }      // padding sorts last
     __syncthreads();
 
     // ---- 3. bitonic sort by (key, index) -------------------------------------------------------------------------------
@@ -142,7 +158,7 @@ int tgn_crop_knn(int B, int N, int Q, int k, const float* xyz, const float* cent
     if (B > 65535) { set_error("crop_knn: B=%d exceeds gridDim.y", B); return TGN_ERR_INVALID; }
     int kpad = 2;
     while (kpad < k) kpad <<= 1;
-    const size_t smem = static_cast<size_t>(kpad) * (sizeof(unsigned long long) + 2 * sizeof(int));
+    const size_t smem = static_cast<size_t>(kpad) * (sizeof(unsigned long long) + sizeof(int));
     int rc = idx64 ? ensure_dynamic_smem(reinterpret_cast<const void*>(crop_knn_kernel<long long>), smem)
                    : ensure_dynamic_smem(reinterpret_cast<const void*>(crop_knn_kernel<int>), smem);
     if (rc != TGN_OK) return rc;

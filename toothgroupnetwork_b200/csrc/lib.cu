@@ -35,7 +35,8 @@ int check_launch(const char* what)
 }
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per (device, kernel): remember the largest value configured for
-// each pair (thread-safe) so that a process touching several GPUs configures every one of them.
+// each pair (thread-safe) so that a process touching several GPUs configures every one of them.  Without the opt-in a
+// kernel's static and dynamic shared memory together must fit in 48 KB, so the kernel's static size counts.
 int ensure_dynamic_smem(const void* func, size_t bytes)
 {
     static std::mutex mu;
@@ -44,7 +45,10 @@ int ensure_dynamic_smem(const void* func, size_t bytes)
     if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); dev = 0; }
     std::lock_guard<std::mutex> lock(mu);
     size_t& have = configured[{dev, func}];
-    if (bytes <= have || bytes <= 48 * 1024) return TGN_OK;
+    if (bytes <= have) return TGN_OK;
+    cudaFuncAttributes attr{};
+    if (cudaFuncGetAttributes(&attr, func) != cudaSuccess) { set_error("cudaFuncGetAttributes: %s", cudaGetErrorString(cudaGetLastError())); return TGN_ERR_CUDA; }
+    if (attr.sharedSizeBytes + bytes <= 48 * 1024) { have = bytes; return TGN_OK; }
     const cudaError_t e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(%zu bytes): %s", bytes, cudaGetErrorString(e)); return TGN_ERR_CUDA; }
     have = bytes;
