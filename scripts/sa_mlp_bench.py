@@ -1,12 +1,12 @@
 """The group-MLP stage of bench.py on its own: ``pn2.sa_group_mlp_max`` (gather -> 9->[32,32,64] -> max over K) at the
-bench shape (B = 1056 clouds, S = 1024, K = 32), on the 3xTF32 tensor-core engine in full-size (TC) and half-size
+bench shape (B = 1056 clouds, S = 1024, K = 32), on the split-fp16 tensor-core engine in full-size (TC) and half-size
 (TC_HALF) CTAs and on the exact-fp32 CUDA-core engine.  ``gidx`` and ``new_xyz`` come from the real FPS + ball query
 on bench.py's own clouds and module.
 
 Each engine is warmed up, then timed with CUDA events over --windows windows of --launches back-to-back launches;
-the median window is reported as ms per launch, with useful TFLOP/s (2 * rows * sum C_l * C_l+1), issued TF32
-TFLOP/s (the 3xTF32 engine's padded MMAs) and that rate as a fraction of the H100 SXM data-sheet dense TF32
-peak (495 TFLOP/s at 700 W).  The card's name, power limit and max SM clock are read in the same run.
+the median window is reported as ms per launch, with useful TFLOP/s (2 * rows * sum C_l * C_l+1), issued FP16
+TFLOP/s (the split-fp16 engine's padded MMAs, no tile falling back to 3xTF32) and that rate as a fraction of the H100 SXM
+data-sheet dense FP16 peak (989 TFLOP/s at 700 W).  The card's name, power limit and max SM clock are read in the same run.
 
     python scripts/sa_mlp_bench.py [--clouds B] [--windows 7] [--launches 20]
 """
@@ -25,7 +25,7 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402  (the workload's constants, clouds and module)
 from toothgroupnetwork_b200 import pointnet2_utils as pn2  # noqa: E402
 
-TF32_PEAK_TFLOPS = 495.0          # H100 SXM data sheet, dense TF32, 700 W
+F16_PEAK_TFLOPS = 989.0           # H100 SXM data sheet, dense FP16, 700 W
 
 
 def card():
@@ -38,14 +38,14 @@ def card():
         return {"name": torch.cuda.get_device_name(), "power_limit": f"unknown ({e!r})"[:80], "max_sm_clock": "unknown"}
 
 
-def issued_tf32_macs_per_row(channels):
-    """TF32 MACs the tensor engine issues per grouped row, all three 3xTF32 terms included.  Every layer runs transposed
-    (weights on M, the tile's rows on N).  The inner layers run on 64 weight rows at K = C_0 rounded up to 8, then the
-    previous width rounded up to 16; at inner widths up to 32 the rows pack W_hi and W_lo of a channel (two MMAs per K-step),
+def issued_f16_macs_per_row(channels):
+    """FP16 MACs the tensor engine issues per grouped row, every split-fp16 term included.  Every layer runs transposed
+    (weights on M, the tile's rows on N).  The inner layers run on 64 weight rows at K = C_0 rounded up to 16, then the
+    previous width rounded up to 16; at inner widths up to 32 the rows pack W_hi and W_lo' of a channel (two MMAs per K-step),
     wider ones hold one channel per row (three).  The last layer runs in 64-channel slices, three MMAs per K-step."""
     L = len(channels) - 1
     np_ = max([16] + [(c + 15) // 16 * 16 for c in channels[1:L]])
-    kpad = [(channels[0] + 7) // 8 * 8] + [(c + 15) // 16 * 16 for c in channels[1:L]]
+    kpad = [(channels[0] + 15) // 16 * 16] + [(c + 15) // 16 * 16 for c in channels[1:L]]
     inner = sum(k * 64 * (2 if np_ <= 32 else 3) for k in kpad[:L - 1])
     return inner + kpad[L - 1] * 64 * 3 * ((channels[L] + 63) // 64)
 
@@ -91,7 +91,7 @@ def main():
     channels = [9] + list(bench.MLP)
     rows = B * S * K
     useful = 2.0 * rows * sum(a * b for a, b in zip(channels[:-1], channels[1:]))
-    issued = 2.0 * rows * issued_tf32_macs_per_row(channels)
+    issued = 2.0 * rows * issued_f16_macs_per_row(channels)
     outs, result = {}, {"card": card(), "shape": {"B": B, "S": S, "K": K, "channels": channels}, "engines": {}}
     for name, engine in (("TC", pn2.ENGINE_TC), ("TC_HALF", pn2.ENGINE_TC_HALF), ("FP32", pn2.ENGINE_FP32)):
         out = torch.empty((B, channels[-1], S), device=dev)
@@ -100,8 +100,8 @@ def main():
         outs[name] = out
         rec = {"ms": med, "windows_ms": [round(m, 4) for m in ms], "useful_tflops": useful / (med * 1e-3) / 1e12}
         if name != "FP32":
-            rec["issued_tf32_tflops"] = issued / (med * 1e-3) / 1e12
-            rec["frac_of_tf32_peak"] = rec["issued_tf32_tflops"] / TF32_PEAK_TFLOPS
+            rec["issued_f16_tflops"] = issued / (med * 1e-3) / 1e12
+            rec["frac_of_f16_peak"] = rec["issued_f16_tflops"] / F16_PEAK_TFLOPS
         result["engines"][name] = rec
     ref = outs["FP32"].double()
     floor = 0.05 * float(ref.abs().max())
@@ -110,12 +110,12 @@ def main():
 
     c = result["card"]
     print(f"# {c['name']}, power limit {c['power_limit']}, max SM clock {c['max_sm_clock']}; B={B} S={S} K={K} {channels}")
-    print(f"# useful {useful / 1e9:.1f} GFLOP, issued 3xTF32 {issued / 1e9:.1f} GFLOP per launch")
-    print("| engine | ms (median) | useful TFLOP/s | issued TF32 TFLOP/s | of 495 |")
+    print(f"# useful {useful / 1e9:.1f} GFLOP, issued split-fp16 {issued / 1e9:.1f} GFLOP per launch")
+    print("| engine | ms (median) | useful TFLOP/s | issued FP16 TFLOP/s | of 989 |")
     print("|---|---|---|---|---|")
     for name, rec in result["engines"].items():
-        print(f"| {name} | {rec['ms']:.3f} | {rec['useful_tflops']:.1f} | {rec.get('issued_tf32_tflops', float('nan')):.1f} | "
-              f"{rec.get('frac_of_tf32_peak', float('nan')):.3f} |")
+        print(f"| {name} | {rec['ms']:.3f} | {rec['useful_tflops']:.1f} | {rec.get('issued_f16_tflops', float('nan')):.1f} | "
+              f"{rec.get('frac_of_f16_peak', float('nan')):.3f} |")
     print(json.dumps(result))
 
 

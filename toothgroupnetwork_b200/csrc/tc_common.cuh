@@ -62,9 +62,10 @@ __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t a) {
 // neighbourhood of K consecutive rows, then + bias and ReLU (both monotone, so they commute with the max), stored
 // channel-first.  `ch0` is this thread's first channel (the second is ch0 + 8).  When K is a multiple of 8 a
 // neighbourhood is whole 8-column blocks of the fragment: one running max per thread, flushed at block boundaries.
-// Any other K takes one pass over the thread's 32 columns per neighbourhood.
+// Any other K takes one pass over the thread's 32 columns per neighbourhood.  `scale` (a power of two) multiplies the max
+// before the bias: an accumulator that holds a scaled product is scaled back once per output instead of once per entry.
 __device__ __forceinline__ void store_neighbourhood_max(const float (&d)[64], int ch0, int cout, const float* __restrict__ bias,
-                                                        float* out_b, int S, int s0, int K, int groups)
+                                                        float* out_b, int S, int s0, int K, int groups, float scale = 1.f)
 {
     const int lane = threadIdx.x & 31;
     const bool ok0 = ch0 < cout, ok1 = ch0 + 8 < cout;
@@ -87,8 +88,8 @@ __device__ __forceinline__ void store_neighbourhood_max(const float (&d)[64], in
             m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
             m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
             if ((lane & 3) == 0) {
-                if (ok0) out_b[static_cast<size_t>(ch0) * S + s0 + sg] = fmaxf(m0 + b0, 0.f);
-                if (ok1) out_b[static_cast<size_t>(ch0 + 8) * S + s0 + sg] = fmaxf(m1 + b1, 0.f);
+                if (ok0) out_b[static_cast<size_t>(ch0) * S + s0 + sg] = fmaxf(fmaf(m0, scale, b0), 0.f);
+                if (ok1) out_b[static_cast<size_t>(ch0 + 8) * S + s0 + sg] = fmaxf(fmaf(m1, scale, b1), 0.f);
             }
         }
         return;
@@ -106,8 +107,8 @@ __device__ __forceinline__ void store_neighbourhood_max(const float (&d)[64], in
             m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
             m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
             if ((lane & 3) == 0 && sg < groups) {
-                if (ok0) out_b[static_cast<size_t>(ch0) * S + s0 + sg] = fmaxf(m0 + b0, 0.f);
-                if (ok1) out_b[static_cast<size_t>(ch0 + 8) * S + s0 + sg] = fmaxf(m1 + b1, 0.f);
+                if (ok0) out_b[static_cast<size_t>(ch0) * S + s0 + sg] = fmaxf(fmaf(m0, scale, b0), 0.f);
+                if (ok1) out_b[static_cast<size_t>(ch0 + 8) * S + s0 + sg] = fmaxf(fmaf(m1, scale, b1), 0.f);
             }
             m0 = m1 = -INFINITY;
             nb = 0;
