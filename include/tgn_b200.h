@@ -407,6 +407,39 @@ int tgn_pw_fill(float *ptr, long long n, float value, void *stream);
 /* out[b*cout + c] = sum_k w[c*w_row_stride + k] * g[b*g_batch_stride + k], k < cin, accumulated in fp64 and rounded once */
 int tgn_pw_cloud_bias(int B, int cout, int cin, const float *w, long long w_row_stride, const float *g, long long g_batch_stride,
                       float *out, void *stream);
+/* The point-transformer decoder's final BatchNorm with TransitionUp's interpolated addend (pt_head.cu; blocks.py:109-110):
+ *   out[r, c] = act(scale_c * src[c, r] + shift_c) + (((0 + f[i0, c] * w0) + f[i1, c] * w1) + f[i2, c] * w2),
+ *   (i_j, w_j) = (idx[3 r + j], w[3 r + j]), every product and sum rounded on its own: pointops.interpolation's torch loop
+ *   followed by the add, in torch's order.  `apply` carries rows, channels, src (channels, rows), the BatchNorm (affine,
+ *   stats, stat_rows, gamma ... momentum, update_running) and the activation (relu / act) exactly as for tgn_pw_apply; its
+ *   rows_per_batch, out_channels and out_c_offset are not used, ymin must be NULL, and out is (rows, channels) ROW-MAJOR.
+ *   f == NULL: no addend (a row-major tgn_pw_apply).  f is (f_rows, channels) row-major; idx entries must lie in [0, f_rows). */
+typedef struct {
+    tgn_pw_apply_t apply;
+    const float *f;
+    const int *idx;
+    const float *w;
+    int f_rows;
+} tgn_pt_up_apply_t;
+int tgn_pt_up_apply(const tgn_pt_up_apply_t *p, void *stream);
+
+/* MultiHead's concat-and-classify (heads.py:53-60 with combine = concat) without the upsampled copies:
+ *   out[r, j] = b[j] + sum_s sum_{c<32} W[j, 32 s + c] * lat_s[c, nn_s[r]],   r < n0, j < k
+ * lat_s: level s's latent, (32, n[s]) channel-major; nn_s: (n0) int32, the k = 1 neighbour of each level-0 point in level s,
+ * or NULL for the identity (n[s] == n0).  W (k, 32 levels) row-major, b (k) or NULL; out (n0, k) row-major.  fp32 FFMA from
+ * +0 in increasing column order, then + b[j].  1 <= levels <= 8, 1 <= k <= 32; nn entries must lie in [0, n[s]). */
+#define TGN_HEAD_MAX_LEVELS 8
+typedef struct {
+    int n0, k, levels;
+    const float *lat[TGN_HEAD_MAX_LEVELS];
+    const int *nn[TGN_HEAD_MAX_LEVELS];
+    int n[TGN_HEAD_MAX_LEVELS];
+    const float *w, *b;
+    float *out;
+} tgn_head_classify_t;
+int tgn_head_classify(const tgn_head_classify_t *p, void *stream);
+int tgn_pt_head_struct_size(int which);    /* sizeof(tgn_pt_up_apply_t) (0) / sizeof(tgn_head_classify_t) (1): binding self-check */
+
 /* PointNet's per-cloud transforms (pw_transform.cu): out[b, j, n] = sum_{i < ct} x[b, i, n] * t[b*t_batch_stride + i*ct + j] for
  * j < ct (fp32 FFMA from +0 in increasing i), and out[b, ct + c, n] = x[b, ct + c, n] bit for bit for c < cpass.  x and out are
  * addressed through (batch, channel, point) element strides and must not overlap.  1 <= ct <= 128. */

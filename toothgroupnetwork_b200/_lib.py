@@ -56,6 +56,8 @@ _SIGS = {
     "tgn_pw_layer_forward": [_vp, _vp],
     "tgn_pw_apply": [_vp, _vp],
     "tgn_pw_fill": [_vp, ctypes.c_longlong, _f, _vp],
+    "tgn_pt_up_apply": [_vp, _vp],
+    "tgn_head_classify": [_vp, _vp],
     "tgn_pw_cloud_bias": [_i, _i, _i, _vp, ctypes.c_longlong, _vp, ctypes.c_longlong, _vp, _vp],
     "tgn_pw_cloud_transform": [_i, _i, _i, _i, _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, ctypes.c_longlong,
                                _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp],
@@ -98,6 +100,23 @@ class PwApply(ctypes.Structure):
     ]
 
 
+class PtUpApply(ctypes.Structure):
+    """tgn_pt_up_apply_t (include/tgn_b200.h)."""
+    _fields_ = [("apply", PwApply), ("f", _vp), ("idx", _vp), ("w", _vp), ("f_rows", _i)]
+
+
+HEAD_MAX_LEVELS = 8
+
+
+class HeadClassify(ctypes.Structure):
+    """tgn_head_classify_t (include/tgn_b200.h)."""
+    _fields_ = [
+        ("n0", _i), ("k", _i), ("levels", _i),
+        ("lat", _vp * HEAD_MAX_LEVELS), ("nn", _vp * HEAD_MAX_LEVELS), ("n", _i * HEAD_MAX_LEVELS),
+        ("w", _vp), ("b", _vp), ("out", _vp),
+    ]
+
+
 class PtLayer(ctypes.Structure):
     """tgn_pt_layer_t (include/tgn_b200.h)."""
     _fields_ = [
@@ -122,7 +141,7 @@ REFERENCE_LAUNCHERS = [
     "subtraction_forward_cuda_launcher", "subtraction_backward_cuda_launcher",
     "aggregation_forward_cuda_launcher", "aggregation_backward_cuda_launcher",
 ]
-EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes", "tgn_kdtree_nodes", "tgn_kdtree_bytes", "tgn_kdtree_radius"]
+EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_pt_head_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes", "tgn_kdtree_nodes", "tgn_kdtree_bytes", "tgn_kdtree_radius"]
 
 
 class TgnError(RuntimeError):
@@ -167,9 +186,13 @@ def load() -> ctypes.CDLL:
     lib.tgn_pw_struct_size.argtypes = [_i]
     lib.tgn_pw_struct_size.restype = _i
     lib.tgn_pt_layer_struct_size.restype = _i
+    lib.tgn_pt_head_struct_size.argtypes = [_i]
+    lib.tgn_pt_head_struct_size.restype = _i
     if (lib.tgn_pw_struct_size(0) != ctypes.sizeof(PwLayer) or lib.tgn_pw_struct_size(1) != ctypes.sizeof(PwApply)
             or lib.tgn_pt_layer_struct_size() != ctypes.sizeof(PtLayer)):
         raise TgnError("ctypes mirror of tgn_pw_layer_t / tgn_pw_apply_t / tgn_pt_layer_t is out of date with include/tgn_b200.h")
+    if lib.tgn_pt_head_struct_size(0) != ctypes.sizeof(PtUpApply) or lib.tgn_pt_head_struct_size(1) != ctypes.sizeof(HeadClassify):
+        raise TgnError("ctypes mirror of tgn_pt_up_apply_t / tgn_head_classify_t is out of date with include/tgn_b200.h")
     _lib = lib
     return lib
 

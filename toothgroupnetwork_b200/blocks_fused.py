@@ -155,3 +155,188 @@ def accelerate(blocks_module) -> None:
 
     ptl.forward, tdc.forward = ptl_forward, td_forward
     ptl._tgn_fused = True
+
+
+# ------------------------------------------------------------------ decoder and heads (blocks.py:82-111, heads.py:13-61)
+
+def _is_lbr(seq, bn: bool) -> bool:
+    """seq is exactly Linear [+ BatchNorm1d] + ReLU, float32"""
+    kinds = [torch.nn.Linear] + ([torch.nn.BatchNorm1d] if bn else []) + [torch.nn.ReLU]
+    if not isinstance(seq, torch.nn.Sequential) or len(seq) != len(kinds) or not all(type(m) is k for m, k in zip(seq, kinds)):
+        return False
+    return seq[0].weight.dtype == torch.float32 and (not bn or _bn_ok(seq[1]))
+
+
+def transition_up_structure_ok(tu, head: bool, c_in: int, c_skip: int = 0) -> bool:
+    """TransitionUp's layers as blocks.py:84-90 builds them, for inputs of c_in channels (the head form's x, or x2) and c_skip (x1)"""
+    lin1, lin2 = tu.linear1, tu.linear2
+    if not (_is_lbr(lin1, True) and _is_lbr(lin2, not head)):
+        return False
+    c = lin1[0].out_features
+    if head:
+        return lin1[0].in_features == 2 * c_in and c == c_in and lin2[0].in_features == c_in and lin2[0].out_features == c_in
+    return lin2[0].in_features == c_in and lin2[0].out_features == c and lin1[0].in_features == c_skip
+
+
+def _cuda_f32(*ts) -> bool:
+    return all(t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 for t in ts)
+
+
+def transition_up_fusable(tu, pxo1, pxo2=None) -> bool:
+    """The fused TransitionUp runs without autograd, on CUDA float32, with the reference's layers; the head form also needs clouds
+    of equal size (its per-cloud bias is indexed by row // rows_per_batch), which reads the offsets on the host."""
+    if not (_enabled and pn2._pw_enabled):
+        return False
+    p1, x1, o1 = pxo1
+    if pxo2 is None:
+        if not _cuda_f32(x1) or _needs_grad(tu, x1) or not transition_up_structure_ok(tu, True, x1.shape[1]):
+            return False
+        ends = o1.cpu().tolist()
+        return ends[-1] == x1.shape[0] and all(e == (b + 1) * ends[0] for b, e in enumerate(ends))
+    p2, x2, o2 = pxo2
+    if not (_cuda_f32(x1, x2, p1, p2) and o1.dtype == torch.int32 and o2.dtype == torch.int32):
+        return False
+    return not _needs_grad(tu, x1, x2) and transition_up_structure_ok(tu, False, x2.shape[1], x1.shape[1])
+
+
+def _rows_operand(x: torch.Tensor, rows_per_batch: int) -> "L.PwLayer":
+    """layer 0 of a chain reading the (rows, c) matrix x through its strides"""
+    d = L.PwLayer()
+    d.mode, d.rows_per_batch = 0, rows_per_batch
+    d.seg_ptr[0], d.seg_channels[0] = L.ptr(x), x.shape[1]
+    d.seg_batch_stride[0], d.seg_row_stride[0], d.seg_chan_stride[0] = rows_per_batch * x.stride(0), x.stride(0), x.stride(1)
+    return d
+
+
+_tu_state = weakref.WeakKeyDictionary()           # module -> (its chain, linear1's first c columns)
+
+
+def transition_up_forward(tu, pxo1, pxo2=None) -> torch.Tensor:
+    """blocks.TransitionUp.forward (:92-111) on the layer chain -> (n, c) float32.
+
+    * With pxo2: linear2(x2) is written row-major, linear1(x1) runs on the chain, and its last BatchNorm + ReLU adds the k = 3
+      interpolation of linear2(x2) at the positions p1 (``tgn_pt_up_apply``: pointops.interpolation's order, bit for bit given
+      the same linear outputs).  The neighbours and weights are what pointops.interpolation computes, from the shared kNN cache.
+    * Head form: x = [x | linear2(mean of x over its cloud)] per cloud.  The second half is constant over a cloud, so its product
+      with linear1's last c weight columns is one fp64 per-cloud bias (``tgn_pw_cloud_bias``) and the chain only runs linear1's
+      first c columns; linear2 runs as the module's own Linear + ReLU on the B cloud means (computed in float64)."""
+    st = _tu_state.get(tu)
+    if st is None:
+        c = tu.linear1[0].out_features
+        st = _tu_state[tu] = (pn2._PwChain(), pn2._ColumnSlice(tu.linear1[0], 0, c) if pxo2 is None else None)
+    chain, head_cols = st
+    lin1, bn1 = tu.linear1[0], tu.linear1[1]
+    c = lin1.out_features
+    _, x1, o1 = pxo1
+    n1 = x1.shape[0]
+    out = torch.empty((n1, c), dtype=torch.float32, device=x1.device)
+    if pxo2 is None:
+        B = o1.shape[0]
+        rpb = n1 // B
+        g = x1.reshape(B, rpb, c).sum(1, dtype=torch.float64).div_(rpb).float()
+        h = tu.linear2(g).contiguous()
+        w1 = lin1.weight.detach()
+        cloud = torch.empty((B, c), dtype=torch.float32, device=x1.device)
+        L.call("tgn_pw_cloud_bias", B, c, c, L.ptr(w1[:, c:]), w1.stride(0), L.ptr(h), h.stride(0), L.ptr(cloud), L.stream_ptr())
+        d = _rows_operand(x1, rpb)
+        d.cloud_bias = L.ptr(cloud)
+        chain.run([head_cols], [bn1], d, n1, out, 0, 1, up=(None, None, None))
+        return out
+    p1, p2, x2, o2 = pxo1[0].contiguous(), pxo2[0].contiguous(), pxo2[1], pxo2[2]
+    f = torch.empty((x2.shape[0], c), dtype=torch.float32, device=x1.device)
+    chain.run([tu.linear2[0]], [tu.linear2[1]], _rows_operand(x2, x2.shape[0]), x2.shape[0], f, 0, 1, up=(None, None, None))
+    idx, d2 = pointops.knn_packed(3, p2, p1, o2, o1)
+    w = pointops._inverse_distance_weights(torch.sqrt(d2)).contiguous()
+    chain.run([lin1], [bn1], _rows_operand(x1, n1), n1, out, 0, 1, up=(f, idx, w))
+    return out
+
+
+def multi_head_structure_ok(mh) -> bool:
+    """MultiHead as heads.py:14-42 builds it with combine = concat and ftype latent: one Linear + BatchNorm1d + ReLU to 32
+    channels per level (at most 8 levels) and one Linear to at most 32 outputs"""
+    levels = len(mh.ni_list)
+    if not (1 <= levels <= L.HEAD_MAX_LEVELS and len(mh.infer_list) == levels and type(mh.cls) is torch.nn.Linear):
+        return False
+    if mh.cls.in_features != 32 * levels or not (1 <= mh.cls.out_features <= 32) or mh.cls.weight.dtype != torch.float32:
+        return False
+    return all(_is_lbr(f.infer, True) and f.infer[0].out_features == 32 for f in mh.infer_list)
+
+
+def multi_head_fusable(mh, stage_list) -> bool:
+    if not (_enabled and pn2._pw_enabled and multi_head_structure_ok(mh)):
+        return False
+    up0 = stage_list["up"][0]
+    n0 = up0["p_out"].shape[0]
+    feats = []
+    for (n, i), func in zip(mh.ni_list, mh.infer_list):
+        st = stage_list[n][i]
+        x, p, o = st["f_out"], st["p_out"], st["offset"]
+        if not (_cuda_f32(x, p) and o.dtype == torch.int32 and x.shape[1] == func.infer[0].in_features):
+            return False
+        if i == 0 and x.shape[0] != n0:
+            return False
+        feats.append(x)
+    return _cuda_f32(up0["p_out"]) and up0["offset"].dtype == torch.int32 and not _needs_grad(mh, *feats)
+
+
+_mh_chains = weakref.WeakKeyDictionary()
+
+
+def multi_head_forward(mh, stage_list):
+    """heads.MultiHead.forward (:53-61) -> (x (n0, k), stage_list).  Each level's Linear + BatchNorm + ReLU runs on the layer chain
+    into a (32, n_s) channel-major latent, stored back as stage_list[n][i][ftype] (a (n_s, 32) view of it, as the reference
+    stores its output); ``tgn_head_classify`` then gathers every level at the k = 1 neighbours of the level-0 points (the same
+    ``pointops.knn_packed`` search pointops.interpolation(k=1) runs, shared between the heads through its cache) and applies
+    cls, without the upsampled copies or their concatenation."""
+    chain = _mh_chains.get(mh)
+    if chain is None:
+        chain = _mh_chains[mh] = pn2._PwChain()
+    up0 = stage_list["up"][0]
+    p0, o0 = up0["p_out"].contiguous(), up0["offset"]
+    n0 = p0.shape[0]
+    d = L.HeadClassify()
+    d.n0, d.k, d.levels = n0, mh.cls.out_features, len(mh.ni_list)
+    keep = []
+    for s, ((n, i), func) in enumerate(zip(mh.ni_list, mh.infer_list)):
+        st = stage_list[n][i]
+        x = st["f_out"]
+        rows = x.shape[0]
+        lat = torch.empty((1, 32, rows), dtype=torch.float32, device=x.device)
+        chain.run([func.infer[0]], [func.infer[1]], _rows_operand(x, rows), rows, lat, 0, rows)
+        st[mh.ftype] = lat[0].t()
+        nn_idx = None
+        if i != 0:
+            nn_idx, _ = pointops.knn_packed(1, st["p_out"].contiguous(), p0, st["offset"], o0)
+        keep += [lat, nn_idx]
+        d.lat[s], d.nn[s], d.n[s] = L.ptr(lat), L.ptr(nn_idx), rows
+    w = mh.cls.weight.detach().contiguous()
+    b = None if mh.cls.bias is None else mh.cls.bias.detach()
+    out = torch.empty((n0, d.k), dtype=torch.float32, device=p0.device)
+    d.w, d.b, d.out = L.ptr(w), L.ptr(b), L.ptr(out)
+    L.call("tgn_head_classify", ctypes.byref(d), L.stream_ptr())
+    return out, stage_list
+
+
+def accelerate_decoder(blocks_module=None, heads_module=None) -> None:
+    """Wrap TransitionUp.forward of an imported reference ``blocks`` module and MultiHead.forward of its ``heads`` module (either
+    may be None); calls the fused paths do not take, autograd included, run the reference's own code.  Idempotent."""
+    if blocks_module is not None and not getattr(blocks_module.TransitionUp, "_tgn_fused", False):
+        tuc = blocks_module.TransitionUp
+        tu_orig = tuc.forward
+
+        def tu_forward(self, pxo1, pxo2=None):
+            if transition_up_fusable(self, pxo1, pxo2):
+                return transition_up_forward(self, pxo1, pxo2)
+            return tu_orig(self, pxo1, pxo2)
+
+        tuc.forward, tuc._tgn_fused = tu_forward, True
+    if heads_module is not None and not getattr(heads_module.MultiHead, "_tgn_fused", False):
+        mhc = heads_module.MultiHead
+        mh_orig = mhc.forward
+
+        def mh_forward(self, stage_list):
+            if multi_head_fusable(self, stage_list):
+                return multi_head_forward(self, stage_list)
+            return mh_orig(self, stage_list)
+
+        mhc.forward, mhc._tgn_fused = mh_forward, True

@@ -87,6 +87,18 @@ def accelerate_blocks(blocks_module=None) -> None:
     blocks_fused.accelerate(blocks_module)
 
 
+def accelerate_decoder(blocks_module=None, heads_module=None) -> None:
+    """Optional: run the no-grad forwards of the reference's ``TransitionUp`` (both forms) and ``MultiHead``
+    (models/modules/cbl_point_transformer/blocks.py:92-111, heads.py:53-61) on the layer chain and ``csrc/pt_head.cu`` through
+    ``toothgroupnetwork_b200.blocks_fused``; under autograd, and for packed clouds of unequal sizes in the head form, the
+    reference's own code keeps running.  Imports both modules from ``sys.path`` when none is passed."""
+    from . import blocks_fused
+    if blocks_module is None and heads_module is None:
+        blocks_module = importlib.import_module("models.modules.cbl_point_transformer.blocks")
+        heads_module = importlib.import_module("models.modules.cbl_point_transformer.heads")
+    blocks_fused.accelerate_decoder(blocks_module, heads_module)
+
+
 def accelerate_inference_pipeline(module=None) -> None:
     """Optional: run the boundary detection and resampling between the two networks of a tgnet inference
     (``InferencePipeLine.get_boundary_sampled_feats``, inference_pipelines/inference_pipeline_tgn.py:289-330: float64 KDTree kNN,

@@ -473,12 +473,14 @@ class _PwChain:
         desc.in_update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
 
     def run(self, convs, bns, first: "L.PwLayer", rows: int, out: torch.Tensor, out_c_offset: int, rows_per_batch_out: int,
-            group: int = 0, slopes: Optional[Sequence[float]] = None, relu: bool = True) -> None:
+            group: int = 0, slopes: Optional[Sequence[float]] = None, relu: bool = True, up: Optional[tuple] = None) -> None:
         """``first`` describes the operand source of layer 0 (mode / segments / gather fields filled by the
         caller).  group > 0: the last layer reduces max/min over ``group`` consecutive rows (set abstraction)
         and ``out`` is (B, C_total, rows/group/B...); group == 0: ``out`` receives every row (feature propagation).
         ``slopes``: LeakyReLU(slopes[l]) follows BatchNorm l instead of ReLU (DGCNN); None leaves every ReLU launch as it was.
-        ``relu=False``: the last BatchNorm is followed by no activation (PointNet's encoder conv3); ``slopes`` takes precedence."""
+        ``relu=False``: the last BatchNorm is followed by no activation (PointNet's encoder conv3); ``slopes`` takes precedence.
+        ``up=(f, idx, w)``: the last BatchNorm goes through ``tgn_pt_up_apply`` instead, ``out`` is (rows, C) row-major and, unless
+        f is None, receives the k = 3 interpolation of f (TransitionUp, blocks.py:110) added to each row."""
         dev = out.device
         n = len(convs)
         couts = [c.weight.shape[0] for c in convs]
@@ -539,22 +541,29 @@ class _PwChain:
         a.update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
         if slopes is not None:
             a.act, a.act_slope = 1, float(slopes[-1])
-        L.call("tgn_pw_apply", ctypes.byref(a), st)
+        if up is None:
+            L.call("tgn_pw_apply", ctypes.byref(a), st)
+        else:
+            u = L.PtUpApply()
+            u.apply = a
+            f, idx, w = up
+            u.f, u.idx, u.w, u.f_rows = L.ptr(f), L.ptr(idx), L.ptr(w), 0 if f is None else f.shape[0]
+            L.call("tgn_pt_up_apply", ctypes.byref(u), st)
         for b in bns:
             if b.training and b.num_batches_tracked is not None:
                 b.num_batches_tracked.add_(1)
 
 
 class _ColumnSlice:
-    """conv's weight from input channel ``lo`` on, with conv's bias, for the packed-weight cache of ``_PwChain`` (keyed by this
-    object): a layer whose leading input columns are constant over each cloud and are added as a per-cloud bias instead"""
+    """conv's weight columns [lo, hi), with conv's bias, for the packed-weight cache of ``_PwChain`` (keyed by this object): a
+    layer whose other input columns are constant over each cloud and are added as a per-cloud bias instead"""
 
-    def __init__(self, conv, lo: int):
-        self.conv, self.lo, self.bias = conv, lo, conv.bias
+    def __init__(self, conv, lo: int, hi: Optional[int] = None):
+        self.conv, self.lo, self.hi, self.bias = conv, lo, hi, conv.bias
 
     @property
     def weight(self) -> torch.Tensor:
-        return self.conv.weight[:, self.lo:]
+        return self.conv.weight[:, self.lo:self.hi]
 
 
 def _pw_set_abstraction(chain: _PwChain, convs, bns, xyz_t, feats_t, new_xyz_t, gidx, xyz_first: bool, out, c_offset: int) -> None:
