@@ -315,11 +315,16 @@ int tgn_sa_group_mlp_max(int B, int N, int S, int K, int D, const float *xyz, co
  * sum / sum of squares of y; ymax / ymin (cout, rows/group) = extrema over groups of `group` consecutive rows
  * (the max over the K neighbours must wait for the BatchNorm scale's sign, so both are kept); with
  * extrema_atomic != 0 they are merged with atomics into buffers the caller pre-filled with -inf / +inf
- * (required when 128 % group != 0).  w_packed: tgn_pw_pack_weights of the (cout, cin) weight.
+ * (required when 128 % group != 0; when 64 % group != 0 with accum = 1).  w_packed: tgn_pw_pack_weights of the (cout, cin) weight.
+ * accum = 1: promoted accumulation -- 128-row tiles whose tensor-core accumulator is added into an fp32 register total with a
+ * round-to-nearest add every K step (16 values of K) and restarted, so the accumulators' truncation is confined to one
+ * chunk; for layers followed by BatchNorm on running statistics, which does not subtract that truncation again.  The field sits
+ * in what was padding: an all-zero descriptor launches exactly what it did before the field existed.
  * in_update_running != 0 with in_affine == 1 applies torch's momentum update to in_running_mean / _var once. */
 typedef struct {
     int rows, rows_per_batch, cin, cout;
     int mode;
+    int accum;              /* 0: one tensor-core accumulator over all of K; 1: promoted (see above) */
     const float *seg_ptr[2];
     int seg_channels[2];
     long long seg_batch_stride[2], seg_row_stride[2], seg_chan_stride[2];

@@ -72,7 +72,7 @@ _SIGS = {
 class PwLayer(ctypes.Structure):
     """tgn_pw_layer_t (include/tgn_b200.h)."""
     _fields_ = [
-        ("rows", _i), ("rows_per_batch", _i), ("cin", _i), ("cout", _i), ("mode", _i),
+        ("rows", _i), ("rows_per_batch", _i), ("cin", _i), ("cout", _i), ("mode", _i), ("accum", _i),
         ("seg_ptr", _vp * 2), ("seg_channels", _i * 2),
         ("seg_batch_stride", ctypes.c_longlong * 2), ("seg_row_stride", ctypes.c_longlong * 2), ("seg_chan_stride", ctypes.c_longlong * 2),
         ("xyz", _vp), ("feats", _vp), ("new_xyz", _vp), ("gidx", _vp),

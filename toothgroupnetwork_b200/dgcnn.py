@@ -18,7 +18,9 @@ The no-grad forward of the whole model (DESIGN §3.12) runs on the tensor-core l
 
 * ``forward(module, x_in)`` -- ``DGCnnModule.forward`` (models/modules/dgcnn.py:96-134) without the (B, 2C, N, k) edge tensors;
 * ``fusable(module, x_in)`` -- whether ``forward`` takes the call;
-* ``accelerate_forward(module_or_class)`` -- wraps ``DGCnnModule.forward``; under autograd the reference's own code runs.
+* ``eval_fusable(module, x_in)`` -- the same, with BatchNorms on running statistics (eval mode) allowed too;
+* ``accelerate_forward(module_or_class, running_stats=False)`` -- wraps ``DGCnnModule.forward``; under autograd the reference's
+  own code runs, and eval-mode calls only reach ``forward`` with ``running_stats=True``.
 """
 from __future__ import annotations
 
@@ -174,19 +176,30 @@ def fusable(module, x_in) -> bool:
     sem pipeline runs the model), the input is a CUDA float32 (B, C_in <= 64, N) tensor with N >= module.k and module.k <= 32,
     and the module has the reference's layer structure.  Looks at attributes only.
 
-    Eval-mode BatchNorm is refused: it subtracts running means from conv7 / conv8 outputs whose per-cloud offsets are large,
+    Eval-mode BatchNorm is refused here: it subtracts running means from conv7 / conv8 outputs whose per-cloud offsets are large,
     and the tensor cores' truncating fp32 accumulation then leaves the fused result 2-3x further from float64 than the
-    reference's own fp32 run (DESIGN §3.12)."""
+    reference's own fp32 run (DESIGN §3.12).  ``eval_fusable`` accepts those calls for ``forward(..., promote=True)``."""
+    return _fusable(module, x_in, False)
+
+
+def eval_fusable(module, x_in) -> bool:
+    """``fusable``, with any of the eight BatchNorms allowed to use running statistics (eval mode, or a mix): the calls that
+    ``forward(module, x_in, promote=True)`` takes, its running-statistics layers on promoted accumulation.  Looks at attributes
+    only."""
+    return _fusable(module, x_in, True)
+
+
+def _fusable(module, x_in, running_stats: bool) -> bool:
     try:
         x = x_in[0]
     except (TypeError, IndexError, KeyError):
         return False
     if not torch.is_tensor(x) or not structure_ok(module):
         return False
-    bns = [getattr(module, n)[1] for n in _LAYERS]
-    if any(pn2._PwChain._bn_mode(b) != 1 for b in bns):
+    modes = [pn2._PwChain._bn_mode(getattr(module, n)[1]) for n in _LAYERS]
+    if not running_stats and any(m != 1 for m in modes):
         return False                  # running statistics (eval mode): left to the reference's forward (DESIGN §3.12)
-    if not input_ok(x.is_cuda, x.dtype, tuple(x.shape), module.k, module.conv1[0].in_channels // 2, True):
+    if not input_ok(x.is_cuda, x.dtype, tuple(x.shape), module.k, module.conv1[0].in_channels // 2, 1 in modes):
         return False
     return not _needs_grad(module, x)
 
@@ -201,11 +214,13 @@ def _chain(module):
     return st
 
 
-def forward(module, x_in, knn: Optional[Callable] = None, keep: Optional[dict] = None) -> dict:
+def forward(module, x_in, knn: Optional[Callable] = None, keep: Optional[dict] = None, promote: bool = False) -> dict:
     """``DGCnnModule.forward`` (models/modules/dgcnn.py:96-134) under no_grad, on csrc/pw_mlp.cu.  ``x_in[0]`` is (B, C_in, N)
     float32 CUDA in any layout; returns ``{"cls_pred": (B, n_cls, N)}``.  BatchNorm keeps torch's semantics: batch statistics in
     train mode, with the running statistics and ``num_batches_tracked`` updated, running statistics in eval mode (which
-    ``fusable`` does not send here).
+    ``fusable`` does not send here), each layer as its own BatchNorm's mode says.  ``promote=True`` runs every layer whose
+    BatchNorm uses running statistics on promoted accumulation (``_PwChain.run``), which keeps eval-mode outputs within the
+    reference fp32 run's distance from float64 (DESIGN §3.12); batch-statistics layers launch the same either way.
 
     * kNN: ``knn_features`` on the current features, three times.
     * EdgeConv: layer 0 gathers [x_j - x_i | x_i] itself, the last layer keeps the max and the min over the k neighbours, and the
@@ -242,7 +257,7 @@ def forward(module, x_in, knn: Optional[Callable] = None, keep: Optional[dict] =
             d.edge_stride[0], d.edge_stride[1], d.edge_stride[2] = src.stride()
             d.gidx, d.N, d.K = L.ptr(gidx), N, k
             seqs = [getattr(module, n) for n in names]
-            chain.run([s[0] for s in seqs], [s[1] for s in seqs], d, B * N * k, feats, off, N, group=k, slopes=[slope[n] for n in names])
+            chain.run([s[0] for s in seqs], [s[1] for s in seqs], d, B * N * k, feats, off, N, group=k, slopes=[slope[n] for n in names], promote=promote)
             src = feats[:, off:off + width]
             off += width
         c6 = module.conv6[0].out_channels
@@ -251,7 +266,7 @@ def forward(module, x_in, knn: Optional[Callable] = None, keep: Optional[dict] =
         d.seg_ptr[0], d.seg_channels[0] = L.ptr(feats), off
         d.seg_batch_stride[0], d.seg_row_stride[0], d.seg_chan_stride[0] = off * N, 1, N
         g = torch.empty((B, c6, 1), dtype=torch.float32, device=dev)
-        chain.run([module.conv6[0]], [module.conv6[1]], d, B * N, g, 0, 1, group=N, slopes=[slope["conv6"]])
+        chain.run([module.conv6[0]], [module.conv6[1]], d, B * N, g, 0, 1, group=N, slopes=[slope["conv6"]], promote=promote)
         w7 = module.conv7[0].weight.detach()
         c7 = w7.shape[0]
         w7 = w7.reshape(c7, -1)
@@ -264,26 +279,33 @@ def forward(module, x_in, knn: Optional[Callable] = None, keep: Optional[dict] =
         d.cloud_bias = L.ptr(cloud)
         h = torch.empty((B, module.conv8[0].out_channels, N), dtype=torch.float32, device=dev)
         chain.run([conv7_x, module.conv8[0]], [module.conv7[1], module.conv8[1]], d, B * N, h, 0, N,
-                  slopes=[slope["conv7"], slope["conv8"]])
+                  slopes=[slope["conv7"], slope["conv8"]], promote=promote)
         if keep is not None:
             keep["x123"], keep["conv8"] = feats, h
         return {"cls_pred": module.cls_conv(module.dp1(h))}
 
 
-def accelerate_forward(module_or_class) -> None:
+def accelerate_forward(module_or_class, running_stats: bool = False) -> None:
     """Wrap ``DGCnnModule.forward`` of an imported reference ``dgcnn`` module (or of the class itself): calls that ``fusable``
     accepts run ``forward``; every other call, autograd included, runs the reference's own forward unchanged -- with whatever
-    ``knn`` the module has, so it composes with ``accelerate``.  Calling it again leaves the class as it is."""
+    ``knn`` the module has, so it composes with ``accelerate``.  ``running_stats=True`` also sends the calls ``eval_fusable``
+    accepts (eval-mode BatchNorm, as in validation) to ``forward(..., promote=True)``.  Calling it again leaves the class as it
+    is, except that ``running_stats=True`` turns the eval-mode routing on."""
     cls = getattr(module_or_class, "DGCnnModule", module_or_class)
     original = cls.forward
     if getattr(original, "_tgn_fused", False):
+        if running_stats:
+            original._tgn_running_stats = True
         return
 
     @functools.wraps(original)
     def fused_forward(self, x_in):
         if fusable(self, x_in):
             return forward(self, x_in)
+        if fused_forward._tgn_running_stats and eval_fusable(self, x_in):
+            return forward(self, x_in, promote=True)
         return original(self, x_in)
 
     fused_forward._tgn_fused = True
+    fused_forward._tgn_running_stats = bool(running_stats)
     cls.forward = fused_forward

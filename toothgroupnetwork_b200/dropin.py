@@ -139,26 +139,32 @@ def accelerate_dgcnn(module=None) -> None:
     dgcnn.accelerate(module)
 
 
-def accelerate_dgcnn_forward(module=None) -> None:
+def accelerate_dgcnn_forward(module=None, running_stats: bool = False) -> None:
     """Optional: run the no-grad forward of the DGCNN model (``DGCnnModule.forward``, models/modules/dgcnn.py:96-134) on the
     tensor-core layer chain of ``toothgroupnetwork_b200.dgcnn``: the EdgeConv gathers, BatchNorm, LeakyReLU and the neighbour max
-    without the (B, 2C, N, k) tensors.  Under autograd the reference's own forward runs.  Imports ``models.modules.dgcnn`` from
-    ``sys.path`` when no module is passed."""
+    without the (B, 2C, N, k) tensors.  Under autograd the reference's own forward runs.  By default only train-mode BatchNorm
+    (batch statistics) takes the fused path; ``running_stats=True`` also sends eval-mode calls (``module.eval()``, as the
+    validation and test phases run) to it, their running-statistics layers on promoted tensor-core accumulation; a later call
+    with True turns that on for an already-wrapped class.  Imports ``models.modules.dgcnn`` from ``sys.path`` when no module is
+    passed."""
     from . import dgcnn
     if module is None:
         module = importlib.import_module("models.modules.dgcnn")
-    dgcnn.accelerate_forward(module)
+    dgcnn.accelerate_forward(module, running_stats=running_stats)
 
 
-def accelerate_pointnet_forward(module=None) -> None:
+def accelerate_pointnet_forward(module=None, running_stats: bool = False) -> None:
     """Optional: run the no-grad forward of the PointNet model (``get_model.forward``, models/modules/pointnet.py:23-35) on the
     tensor-core layer chain of ``toothgroupnetwork_b200.pointnet``: both learned transforms, BatchNorm and the max over the points
     without the (B, 2176, N) concatenation.  ``PointFirstModule`` calls ``get_model``, so the sem pipeline uses it too.  Under
-    autograd the reference's own forward runs.  Imports ``models.modules.pointnet`` from ``sys.path`` when no module is passed."""
+    autograd the reference's own forward runs.  By default only train-mode BatchNorm (batch statistics) takes the fused path;
+    ``running_stats=True`` also sends eval-mode calls (validation and test phases) to it, their running-statistics layers on
+    promoted tensor-core accumulation; a later call with True turns that on for an already-wrapped class.  Imports
+    ``models.modules.pointnet`` from ``sys.path`` when no module is passed."""
     from . import pointnet
     if module is None:
         module = importlib.import_module("models.modules.pointnet")
-    pointnet.accelerate_forward(module)
+    pointnet.accelerate_forward(module, running_stats=running_stats)
 
 
 def uninstall() -> None:

@@ -8,7 +8,9 @@ statistics of all B * N points and updates its running statistics.
 * ``forward(module, x_in)`` -- the same forward without the (B, 2176, N) concatenation, its repeat, or any full-size
   conv3 / BatchNorm output;
 * ``fusable(module, x_in)`` -- whether ``forward`` takes the call;
-* ``accelerate_forward(module_or_class)`` -- wraps ``get_model.forward``; under autograd the reference's own code runs.
+* ``eval_fusable(module, x_in)`` -- the same, with BatchNorms on running statistics (eval mode) allowed too;
+* ``accelerate_forward(module_or_class, running_stats=False)`` -- wraps ``get_model.forward``; under autograd the reference's own
+  code runs, and eval-mode calls only reach ``forward`` with ``running_stats=True``.
 """
 from __future__ import annotations
 
@@ -121,17 +123,30 @@ def fusable(module, x_in) -> bool:
     statistics (train mode, as the sem pipeline runs the model), the input is a CUDA float32 (B, 6, N) tensor, and the module
     has the reference's layer structure.  Looks at attributes only.
 
-    Eval-mode BatchNorm is refused for the reason given for DGCNN (DESIGN §3.12): subtracting running means from layers whose
-    per-cloud offsets are large makes the tensor cores' truncating accumulation visible."""
+    Eval-mode BatchNorm is refused here for the reason given for DGCNN (DESIGN §3.12): subtracting running means from layers
+    whose per-cloud offsets are large makes the tensor cores' truncating accumulation visible.  ``eval_fusable`` accepts those
+    calls for ``forward(..., promote=True)``."""
+    return _fusable(module, x_in, False)
+
+
+def eval_fusable(module, x_in) -> bool:
+    """``fusable``, with any of the twelve BatchNorms allowed to use running statistics (eval mode, or a mix): the calls that
+    ``forward(module, x_in, promote=True)`` takes, its running-statistics layers on promoted accumulation.  Looks at attributes
+    only."""
+    return _fusable(module, x_in, True)
+
+
+def _fusable(module, x_in, running_stats: bool) -> bool:
     try:
         x = x_in[0]
     except (TypeError, IndexError, KeyError):
         return False
     if not torch.is_tensor(x) or not structure_ok(module):
         return False
-    if any(pn2._PwChain._bn_mode(b) != 1 for b in _bns(module)):
+    modes = [pn2._PwChain._bn_mode(b) for b in _bns(module)]
+    if not running_stats and any(m != 1 for m in modes):
         return False
-    if not input_ok(x.is_cuda, x.dtype, tuple(x.shape), True):
+    if not input_ok(x.is_cuda, x.dtype, tuple(x.shape), 1 in modes):
         return False
     return not _needs_grad(module, x)
 
@@ -172,14 +187,14 @@ def cloud_transform(x: torch.Tensor, t: torch.Tensor, out: torch.Tensor) -> torc
     return out
 
 
-def _stn(chain, stn, src: torch.Tensor) -> torch.Tensor:
+def _stn(chain, stn, src: torch.Tensor, promote: bool) -> torch.Tensor:
     """STN3d / STNkd.forward (pointnet_utils.py:27-45, 68-85) on src (B, C, N): the conv chain keeps only each cloud's extrema
     over its N points, the apply writes relu(bn3(max)) (B, 1024); the fc layers run as the module's own, in the reference's
     expression order"""
     B, _, N = src.shape
     c3 = stn.conv3.out_channels
     g = torch.empty((B, c3, 1), dtype=torch.float32, device=src.device)
-    chain.run([stn.conv1, stn.conv2, stn.conv3], [stn.bn1, stn.bn2, stn.bn3], _source(src), B * N, g, 0, 1, group=N)
+    chain.run([stn.conv1, stn.conv2, stn.conv3], [stn.bn1, stn.bn2, stn.bn3], _source(src), B * N, g, 0, 1, group=N, promote=promote)
     x = g.view(-1, c3)
     x = F.relu(stn.bn4(stn.fc1(x)))
     x = F.relu(stn.bn5(stn.fc2(x)))
@@ -190,10 +205,13 @@ def _stn(chain, stn, src: torch.Tensor) -> torch.Tensor:
     return x.view(-1, k, k)
 
 
-def forward(module, x_in, keep: Optional[dict] = None):
+def forward(module, x_in, keep: Optional[dict] = None, promote: bool = False):
     """``get_model.forward`` (models/modules/pointnet.py:23-35) under no_grad, on csrc/pw_mlp.cu and csrc/pw_transform.cu.
     ``x_in[0]`` is (B, 6, N) float32 CUDA in any layout; returns ``(log-probabilities (B, k, N), trans_feat (B, 128, 128))``.
-    BatchNorm keeps torch's semantics: batch statistics, running statistics and ``num_batches_tracked`` updated once per layer.
+    BatchNorm keeps torch's semantics, each layer as its own BatchNorm's mode says: batch statistics, running statistics and
+    ``num_batches_tracked`` updated once per layer in train mode; running statistics, untouched, in eval mode.  ``promote=True``
+    runs every layer whose BatchNorm uses running statistics on promoted accumulation (``_PwChain.run``, DESIGN §3.15); layers
+    on batch statistics launch the same either way.
 
     * STN3d: three layers read x through its strides, the last keeps only each cloud's max and min over its N points, and one
       apply writes relu(bn3(max)); fc1-fc3 and the identity run as the module's own layers -> trans.
@@ -213,18 +231,18 @@ def forward(module, x_in, keep: Optional[dict] = None):
     rows = B * N
     dev = x.device
     with torch.no_grad():
-        trans = _stn(chain, feat.stn, x)
+        trans = _stn(chain, feat.stn, x, promote)
         xt = cloud_transform(x, trans, torch.empty((B, C, N), dtype=torch.float32, device=dev))
         c1 = feat.conv1.out_channels
         a1 = torch.empty((B, c1, N), dtype=torch.float32, device=dev)
-        chain.run([feat.conv1], [feat.bn1], _source(xt), rows, a1, 0, N)
+        chain.run([feat.conv1], [feat.bn1], _source(xt), rows, a1, 0, N, promote=promote)
         del xt
-        trans_feat = _stn(chain, feat.fstn, a1)
+        trans_feat = _stn(chain, feat.fstn, a1, promote)
         pointfeat = cloud_transform(a1, trans_feat, torch.empty((B, c1, N), dtype=torch.float32, device=dev))
         del a1
         c3 = feat.conv3.out_channels
         g = torch.empty((B, c3, 1), dtype=torch.float32, device=dev)
-        chain.run([feat.conv2, feat.conv3], [feat.bn2, feat.bn3], _source(pointfeat), rows, g, 0, 1, group=N, relu=False)
+        chain.run([feat.conv2, feat.conv3], [feat.bn2, feat.bn3], _source(pointfeat), rows, g, 0, 1, group=N, relu=False, promote=promote)
         w1 = module.conv1.weight.detach()
         co = w1.shape[0]
         w1 = w1.reshape(co, -1)
@@ -233,7 +251,7 @@ def forward(module, x_in, keep: Optional[dict] = None):
         d = _source(pointfeat)
         d.cloud_bias = L.ptr(cloud)
         h = torch.empty((B, module.conv3.out_channels, N), dtype=torch.float32, device=dev)
-        chain.run([head1, module.conv2, module.conv3], [module.bn1, module.bn2, module.bn3], d, rows, h, 0, N)
+        chain.run([head1, module.conv2, module.conv3], [module.bn1, module.bn2, module.bn3], d, rows, h, 0, N, promote=promote)
         if keep is not None:
             keep.update(trans=trans, g=g.view(B, c3), pointfeat=pointfeat, head3=h)
         out = module.conv4(h)
@@ -243,20 +261,27 @@ def forward(module, x_in, keep: Optional[dict] = None):
         return out, trans_feat
 
 
-def accelerate_forward(module_or_class) -> None:
+def accelerate_forward(module_or_class, running_stats: bool = False) -> None:
     """Wrap ``get_model.forward`` of an imported reference ``pointnet`` module (or of the class itself): calls that ``fusable``
-    accepts run ``forward``; every other call, autograd included, runs the reference's own forward unchanged.  Calling it again
-    leaves the class as it is."""
+    accepts run ``forward``; every other call, autograd included, runs the reference's own forward unchanged.
+    ``running_stats=True`` also sends the calls ``eval_fusable`` accepts (eval-mode BatchNorm, as in validation) to
+    ``forward(..., promote=True)``.  Calling it again leaves the class as it is, except that ``running_stats=True`` turns the
+    eval-mode routing on."""
     cls = getattr(module_or_class, "get_model", module_or_class)
     original = cls.forward
     if getattr(original, "_tgn_fused", False):
+        if running_stats:
+            original._tgn_running_stats = True
         return
 
     @functools.wraps(original)
     def fused_forward(self, x_in):
         if fusable(self, x_in):
             return forward(self, x_in)
+        if fused_forward._tgn_running_stats and eval_fusable(self, x_in):
+            return forward(self, x_in, promote=True)
         return original(self, x_in)
 
     fused_forward._tgn_fused = True
+    fused_forward._tgn_running_stats = bool(running_stats)
     cls.forward = fused_forward

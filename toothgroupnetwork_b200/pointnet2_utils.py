@@ -473,14 +473,18 @@ class _PwChain:
         desc.in_update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
 
     def run(self, convs, bns, first: "L.PwLayer", rows: int, out: torch.Tensor, out_c_offset: int, rows_per_batch_out: int,
-            group: int = 0, slopes: Optional[Sequence[float]] = None, relu: bool = True, up: Optional[tuple] = None) -> None:
+            group: int = 0, slopes: Optional[Sequence[float]] = None, relu: bool = True, up: Optional[tuple] = None,
+            promote: bool = False) -> None:
         """``first`` describes the operand source of layer 0 (mode / segments / gather fields filled by the
         caller).  group > 0: the last layer reduces max/min over ``group`` consecutive rows (set abstraction)
         and ``out`` is (B, C_total, rows/group/B...); group == 0: ``out`` receives every row (feature propagation).
         ``slopes``: LeakyReLU(slopes[l]) follows BatchNorm l instead of ReLU (DGCNN); None leaves every ReLU launch as it was.
         ``relu=False``: the last BatchNorm is followed by no activation (PointNet's encoder conv3); ``slopes`` takes precedence.
         ``up=(f, idx, w)``: the last BatchNorm goes through ``tgn_pt_up_apply`` instead, ``out`` is (rows, C) row-major and, unless
-        f is None, receives the k = 3 interpolation of f (TransitionUp, blocks.py:110) added to each row."""
+        f is None, receives the k = 3 interpolation of f (TransitionUp, blocks.py:110) added to each row.
+        ``promote=True``: each layer whose own BatchNorm uses running statistics runs the promoted-accumulation kernel
+        (``accum`` = 1: 128-row tiles, the tensor-core accumulator rounded to nearest into an fp32 total every 16 values of K);
+        layers on batch statistics launch exactly as with False."""
         dev = out.device
         n = len(convs)
         couts = [c.weight.shape[0] for c in convs]
@@ -508,12 +512,13 @@ class _PwChain:
             bias = None if conv.bias is None else conv.bias.detach()
             d.bias = L.ptr(bias)
             d.stats = L.ptr(stats[l])
+            d.accum = 1 if (promote and not train[l]) else 0
             last = l == n - 1
             if last and group > 0:
                 ng = rows // group
                 ymax = torch.empty((cout, ng), dtype=torch.float32, device=dev)
                 ymin = torch.empty((cout, ng), dtype=torch.float32, device=dev)
-                atomic = 1 if (128 % group) != 0 else 0
+                atomic = 1 if ((64 if d.accum else 128) % group) != 0 else 0      # half a tile of rows per epilogue thread
                 if atomic:
                     L.call("tgn_pw_fill", L.ptr(ymax), ymax.numel(), ctypes.c_float(float("-inf")), st)
                     L.call("tgn_pw_fill", L.ptr(ymin), ymin.numel(), ctypes.c_float(float("inf")), st)
