@@ -71,14 +71,18 @@ def test_clustering_host_helpers():
         clustering._as_float32(f32.astype(np.float64) + 1e-12)
 
 
-def test_dbscan_class_refuses_what_it_does_not_implement():
+def test_dbscan_class_refuses_what_it_does_not_implement_from_12_points():
     from toothgroupnetwork_b200 import clustering
     with pytest.raises(clustering.L.TgnError):
         clustering.DBSCAN(eps=0.1, min_samples=3, metric="manhattan")
     with pytest.raises(clustering.L.TgnError):
         clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 2), np.float32))
+    # 12 points: the smallest cloud scikit-learn searches with its KD tree, so the smallest that runs on the device
     if torch.cuda.is_available():
-        assert clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 3), np.float32)).labels_.tolist() == [0, 0, 0, 0]
+        assert clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((12, 3), np.float32)).labels_.tolist() == [0] * 12
     else:
         with pytest.raises(clustering.L.TgnError):                    # no CPU path: the product fails loudly without a GPU
-            clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 3), np.float32))
+            clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((12, 3), np.float32))
+    # up to 11 points scikit-learn searches by brute force, and the fit is its own, on the host, with or without a GPU
+    pytest.importorskip("sklearn.cluster")
+    assert clustering.DBSCAN(eps=0.1, min_samples=3).fit(np.zeros((4, 3), np.float32)).labels_.tolist() == [0, 0, 0, 0]

@@ -5,8 +5,11 @@
 clusters with MeanShift and gives every noise point the majority label of its 10 nearest labelled points (a KDTree).  On a
 trained network the DBSCAN alone costs 0.9 s per cloud on the host -- an order of magnitude more than the two networks.
 
-Here ``dbscan`` is csrc/dbscan.cu (labels and core samples equal to scikit-learn's: same float64 predicate, same cluster
-numbering, same border rule), the noise vote uses the float64 selection kernel of csrc/crop_knn.cu, and
+Here ``dbscan`` is csrc/dbscan.cu (labels and core samples equal to scikit-learn's: the float64 predicate of its KD-tree
+search, (dx^2 + dy^2) + dz^2 <= eps^2, the same cluster numbering, the same border rule).  scikit-learn searches clouds of at
+most 11 points by brute force instead, whose expanded distance can fall on the other side of eps; ``dbscan`` and ``DBSCAN``
+hand those to scikit-learn on the host.  Non-finite coordinates raise scikit-learn's ValueError.  The noise vote uses the
+float64 selection kernel of csrc/crop_knn.cu, and
 ``get_clustering_labels`` keeps the reference's steps and return value.  The elongation test is the reference's (PCA
 eigenvalues of the core points); the MeanShift split of at most three elongated clusters is ``MeanShift`` below, whose seed
 ascent is csrc/meanshift.cu (scikit-learn's seeds, centres and labels bit for bit).  ``accelerate(ops_utils_module)`` swaps the
@@ -40,7 +43,9 @@ def _workspace(n: int, device) -> torch.Tensor:
 
 def dbscan_device(points: torch.Tensor, eps: float = 0.03, min_samples: int = 30) -> Tuple[torch.Tensor, torch.Tensor]:
     """points (n,3) float32 CUDA -> (labels (n) int32, core (n) uint8), both on the device; equal to
-    ``sklearn.cluster.DBSCAN(eps, min_samples).fit(points)``'s ``labels_`` / ``core_sample_indices_``."""
+    ``sklearn.cluster.DBSCAN(eps, min_samples).fit(points)``'s ``labels_`` / ``core_sample_indices_`` wherever scikit-learn
+    takes its KD-tree path (n >= 12).  At every n the kernel applies that path's predicate; a point with a non-finite
+    coordinate is no one's neighbour, not even its own, so it is noise."""
     L.require_cuda(points)
     if points.dim() != 2 or points.shape[1] != 3 or points.dtype != torch.float32:
         raise L.TgnError(f"dbscan expects (n,3) float32 points, got {tuple(points.shape)} {points.dtype}")
@@ -67,9 +72,51 @@ def _as_float32(points: np.ndarray) -> np.ndarray:
     return down
 
 
+def _check_finite(x) -> None:
+    """scikit-learn's refusal of non-finite coordinates (``sklearn.utils.check_array``), with the start of its messages"""
+    if isinstance(x, torch.Tensor):
+        if bool(torch.isfinite(x).all()):
+            return
+        nan, dtype = bool(torch.isnan(x).any()), np.dtype(str(x.dtype).replace("torch.", ""))
+    else:
+        if np.isfinite(x).all():
+            return
+        nan, dtype = bool(np.isnan(x).any()), x.dtype
+    if nan:
+        raise ValueError("Input X contains NaN.")
+    raise ValueError(f"Input X contains infinity or a value too large for {dtype!r}.")
+
+
+# DBSCAN's NearestNeighbors(radius=eps) keeps the default n_neighbors=5, and algorithm="auto" searches by brute force when
+# 5 >= n // 2.  That path compares |x|^2 - 2 x.y + |y|^2 (BLAS norms and a GEMM) with eps^2, not the KD tree's
+# (dx^2 + dy^2) + dz^2, and the two disagree on pairs within rounding of eps: such clouds go to scikit-learn itself.
+_BRUTE_MAX_N = 11
+
+
+def _host_dbscan(X: np.ndarray, eps: float, min_samples: int) -> Tuple[np.ndarray, np.ndarray]:
+    try:
+        from sklearn.cluster import DBSCAN as SkDBSCAN
+    except ImportError as e:
+        raise L.TgnError(f"dbscan: clouds of at most {_BRUTE_MAX_N} points take scikit-learn's brute-force path on the host, "
+                         f"and scikit-learn cannot be imported ({e})") from e
+    DBSCAN.host_fits += 1
+    ref = SkDBSCAN(eps=eps, min_samples=min_samples).fit(X)
+    return ref.labels_.astype(np.int64), ref.core_sample_indices_.astype(np.int64)
+
+
 def dbscan(points, eps: float = 0.03, min_samples: int = 30) -> Tuple[np.ndarray, np.ndarray]:
-    """numpy or tensor (n,3) -> (labels_ int64 (n), core_sample_indices_ int64) like the attributes of a fitted sklearn DBSCAN."""
-    pts = torch.as_tensor(_as_float32(points)) if isinstance(points, np.ndarray) else points.float()
+    """numpy or tensor (n,3) -> (labels_ int64 (n), core_sample_indices_ int64) like the attributes of a fitted sklearn DBSCAN.
+    Non-finite coordinates raise scikit-learn's ValueError; clouds of 1 to 11 points are fitted by scikit-learn on the host."""
+    host = None if isinstance(points, torch.Tensor) else np.asarray(points)
+    pts = points.float() if host is None else host
+    if pts.ndim != 2 or pts.shape[1] != 3:
+        raise L.TgnError(f"dbscan expects (n,3) points, got {tuple(pts.shape)}")
+    _check_finite(pts)
+    if host is not None:
+        pts = torch.as_tensor(_as_float32(host))
+    if 1 <= pts.shape[0] <= _BRUTE_MAX_N:
+        # the caller's array as it is: the brute-force path rounds differently on float32 and float64 input
+        return _host_dbscan(pts.cpu().numpy() if host is None else host, eps, min_samples)
     if not pts.is_cuda and not torch.cuda.is_available():
         raise L.TgnError("dbscan needs a CUDA device (there is no CPU path)")
     pts = pts if pts.is_cuda else pts.cuda()
@@ -81,7 +128,10 @@ def dbscan(points, eps: float = 0.03, min_samples: int = 30) -> Tuple[np.ndarray
 class DBSCAN:
     """The slice of ``sklearn.cluster.DBSCAN`` the reference uses -- ``DBSCAN(eps=..., min_samples=...).fit(X, y)`` then
     ``.labels_`` / ``.core_sample_indices_`` / ``.components_`` -- on csrc/dbscan.cu: ops_utils.py:28,98, tsegnet.py:59,
-    inference_pipeline_tsegnet.py:39.  Euclidean metric only, which is all the reference asks for."""
+    inference_pipeline_tsegnet.py:39.  Euclidean metric only, which is all the reference asks for.  Fits of 1 to 11 points, which
+    scikit-learn searches by brute force, are scikit-learn's own and counted in ``host_fits``."""
+
+    host_fits = 0
 
     def __init__(self, eps: float = 0.5, *, min_samples: int = 5, metric: str = "euclidean", **unsupported):
         if metric != "euclidean" or any(v is not None for v in unsupported.values()):
@@ -125,12 +175,14 @@ def _majority(rows: np.ndarray) -> np.ndarray:
 
 def get_clustering_labels(moved_points, labels):
     """Drop-in for ops_utils.get_clustering_labels (:86-144): moved_points (N,3), labels (N,) or (N,1) semantic classes ->
-    cluster label of every foreground point (labels != 0), int64."""
-    if not torch.cuda.is_available():
-        raise L.TgnError("get_clustering_labels needs a CUDA device (there is no CPU path)")
+    cluster label of every foreground point (labels != 0), int64.  Non-finite foreground coordinates raise scikit-learn's
+    ValueError, as the reference's DBSCAN.fit does."""
     moved_points = np.asarray(moved_points)
     cond = np.asarray(labels) != 0
     fg = moved_points[cond, :]
+    _check_finite(fg)
+    if not torch.cuda.is_available():
+        raise L.TgnError("get_clustering_labels needs a CUDA device (there is no CPU path)")
     fg_dev = torch.as_tensor(_as_float32(fg)).cuda()
     lab_dev, core_dev = dbscan_device(fg_dev, 0.03, 30)
     both = torch.stack([lab_dev, core_dev.int()]).cpu().numpy()
