@@ -402,6 +402,16 @@ int tgn_pt_layer_struct_size(void);
 /* layers with fewer queries than this run one CTA per query instead of one warp per query (default 1024); returns the old value.
  * c = 16 layers always run two queries per warp: the threshold does not apply to them. */
 int tgn_pt_layer_set_cta_threshold(int n_queries);
+/* The same launch with the fp64 batch sums of its output, for the BatchNorm that follows the layer in PointTransformerBlock
+ * (blocks.py:131, bn2): out_stats (2c doubles, ACCUMULATED: caller zeroes) = {sum[ch], sumsq[ch]} of out over its n rows, each
+ * element added to the fp64 sums as it is written.  `layer` is exactly what tgn_pt_layer_forward takes, and out is bit for bit
+ * what that call writes. */
+typedef struct {
+    tgn_pt_layer_t layer;
+    double *out_stats;
+} tgn_pt_layer_sums_t;
+int tgn_pt_layer_forward_sums(const tgn_pt_layer_sums_t *p, void *stream);
+int tgn_pt_layer_sums_struct_size(void);
 
 size_t tgn_pw_packed_bytes(int cout, int cin);
 int tgn_pw_struct_size(int which);         /* sizeof(tgn_pw_layer_t) (0) / sizeof(tgn_pw_apply_t) (1): binding self-check */
@@ -427,6 +437,21 @@ typedef struct {
     int f_rows;
 } tgn_pt_up_apply_t;
 int tgn_pt_up_apply(const tgn_pt_up_apply_t *p, void *stream);
+
+/* PointTransformerBlock's last BatchNorm, residual and ReLU (pt_block.cu; blocks.py:132-134):
+ *   out[r, c] = relu(fl(bn3(src[c, r])) + identity[r, c])
+ * the BatchNorm value rounded to fp32 first (subtract-first, as tgn_pw_apply), then one fp32 add, then the ReLU -- torch's
+ * bn3(...) followed by the in-place += and relu.  `apply` carries rows, channels, src (channels, rows) and the BatchNorm exactly as
+ * for tgn_pw_apply; relu != 0 applies the ReLU after the add; rows_per_batch, out_channels and out_c_offset are not used, ymin must
+ * be NULL and act 0, and out is (rows, channels) ROW-MAJOR.  identity is (rows, channels) row-major with row stride
+ * identity_row_stride (in floats); it is only read and must not overlap out. */
+typedef struct {
+    tgn_pw_apply_t apply;
+    const float *identity;
+    long long identity_row_stride;
+} tgn_pt_res_apply_t;
+int tgn_pt_res_apply(const tgn_pt_res_apply_t *p, void *stream);
+int tgn_pt_res_apply_struct_size(void);    /* sizeof(tgn_pt_res_apply_t): binding self-check */
 
 /* MultiHead's concat-and-classify (heads.py:53-60 with combine = concat) without the upsampled copies:
  *   out[r, j] = b[j] + sum_s sum_{c<32} W[j, 32 s + c] * lat_s[c, nn_s[r]],   r < n0, j < k

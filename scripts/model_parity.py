@@ -2,7 +2,7 @@
 """Model-level parity + timing of the reference's REAL model files on the two operator sets
 (VERDICT r1 item 1; SURVEY.md 8d configs C2-model, C3, C4).
 
-    python scripts/model_parity.py [--out PATH.json] [--points 24000] [--cases pp,tseg,tgn,tgni,tgnb]
+    python scripts/model_parity.py [--out PATH.json] [--points 24000] [--cases pp,tseg,tgn,tgni,tgnb] [--fused-decoder-blocks]
 
 For each case the reference's unmodified ``models/modules/*.py`` is built twice in this process
 (``oracle/ref_models.World``): once on the reference's own operators (verbatim ``pointops`` kernels
@@ -380,6 +380,11 @@ def case_tgn_infer(worlds, feats, labels, train_bn, timer, params=TGN_PARAMS, te
         with w, torch.no_grad():
             torch.manual_seed(0)
             gm = w.mod("models.modules.grouping_network_module")
+            if w.ops == "b200" and FUSED_DECODER_BLOCKS:
+                from toothgroupnetwork_b200 import blocks_fused
+                blk = w.mod("models.modules.cbl_point_transformer.blocks")
+                blocks_fused.accelerate_decoder(blk, w.mod("models.modules.cbl_point_transformer.heads"))
+                blocks_fused.accelerate_blocks(blk)
             module = dev(gm.GroupingNetworkModule({"model_parameter": dict(params)}))
             if state is None:
                 state = {k: v.clone() for k, v in module.state_dict().items()}
@@ -451,8 +456,13 @@ def finish(outs, coords, times):
         c_new, c_ref = coords["b200"], coords["reference"]
         res["sampled_coords_bitwise"] = {k: bool(torch.equal(c_new[k], c_ref[k])) for k in c_ref}
         res["indices_identical"] = bool(all(res["sampled_coords_bitwise"].values()))
+        if "nn_crop_indexes" in ref:
+            res["crop_indexes_identical"] = bool(torch.equal(new["nn_crop_indexes"], ref["nn_crop_indexes"]))
         res["speedup_vs_reference_ops"] = times["reference"] / times["b200"] if times["b200"] > 0 else None
     return res
+
+
+FUSED_DECODER_BLOCKS = False
 
 
 def main():
@@ -461,7 +471,12 @@ def main():
     ap.add_argument("--points", type=int, default=24000)
     ap.add_argument("--cases", default="pp,tseg,tgn,tgni")
     ap.add_argument("--cpu-dry-run", action="store_true")
+    ap.add_argument("--fused-decoder-blocks", action="store_true",
+                    help="tgni / tgnb: also run TransitionUp, MultiHead and PointTransformerBlock on the fused kernels "
+                         "(blocks_fused.accelerate_decoder and accelerate_blocks)")
     args = ap.parse_args()
+    global FUSED_DECODER_BLOCKS
+    FUSED_DECODER_BLOCKS = args.fused_decoder_blocks
 
     if args.cpu_dry_run:
         torch.Tensor.cuda = lambda self, *a, **k: self
@@ -478,7 +493,7 @@ def main():
 
     feats, labels = make_inputs(args.points)
     timer = Timer()
-    report = {"points": args.points, "rel_tol": REL_TOL, "floor": "1e-3 * max|reference tensor|",
+    report = {"points": args.points, "fused_decoder_blocks": FUSED_DECODER_BLOCKS, "rel_tol": REL_TOL, "floor": "1e-3 * max|reference tensor|",
               "precision": "cudnn.allow_tf32=False, cuda.matmul.allow_tf32=False", "device": torch.cuda.get_device_name(0) if torch.cuda.is_available() else "cpu"}
     cases = args.cases.split(",")
     if "pp" in cases:
@@ -497,7 +512,8 @@ def main():
     os.makedirs(os.path.dirname(args.out), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(report, f, indent=1)
-    brief = {k: {kk: v[kk] for kk in ("verdict", "indices_identical", "ms", "speedup_vs_reference_ops", "grads") if kk in v}
+    brief = {k: {kk: v[kk] for kk in ("verdict", "indices_identical", "crop_indexes_identical", "ms", "speedup_vs_reference_ops", "grads")
+                 if kk in v}
              for k, v in report.items() if isinstance(v, dict)}
     print(json.dumps(brief, indent=1))
 

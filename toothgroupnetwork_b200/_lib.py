@@ -57,6 +57,8 @@ _SIGS = {
     "tgn_pw_apply": [_vp, _vp],
     "tgn_pw_fill": [_vp, ctypes.c_longlong, _f, _vp],
     "tgn_pt_up_apply": [_vp, _vp],
+    "tgn_pt_res_apply": [_vp, _vp],
+    "tgn_pt_layer_forward_sums": [_vp, _vp],
     "tgn_head_classify": [_vp, _vp],
     "tgn_pw_cloud_bias": [_i, _i, _i, _vp, ctypes.c_longlong, _vp, ctypes.c_longlong, _vp, _vp],
     "tgn_pw_cloud_transform": [_i, _i, _i, _i, _vp, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, _vp, ctypes.c_longlong,
@@ -105,6 +107,11 @@ class PtUpApply(ctypes.Structure):
     _fields_ = [("apply", PwApply), ("f", _vp), ("idx", _vp), ("w", _vp), ("f_rows", _i)]
 
 
+class PtResApply(ctypes.Structure):
+    """tgn_pt_res_apply_t (include/tgn_b200.h)."""
+    _fields_ = [("apply", PwApply), ("identity", _vp), ("identity_row_stride", ctypes.c_longlong)]
+
+
 HEAD_MAX_LEVELS = 8
 
 
@@ -133,6 +140,11 @@ class PtLayer(ctypes.Structure):
     ]
 
 
+class PtLayerSums(ctypes.Structure):
+    """tgn_pt_layer_sums_t (include/tgn_b200.h)."""
+    _fields_ = [("layer", PtLayer), ("out_stats", _vp)]
+
+
 # the reference's ten extern "C" launchers (part 1): void return, legacy default stream
 REFERENCE_LAUNCHERS = [
     "furthestsampling_cuda_launcher", "knnquery_cuda_launcher",
@@ -141,7 +153,7 @@ REFERENCE_LAUNCHERS = [
     "subtraction_forward_cuda_launcher", "subtraction_backward_cuda_launcher",
     "aggregation_forward_cuda_launcher", "aggregation_backward_cuda_launcher",
 ]
-EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_pt_head_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes", "tgn_kdtree_nodes", "tgn_kdtree_bytes", "tgn_kdtree_radius"]
+EXPORTS = list(_SIGS) + REFERENCE_LAUNCHERS + ["tgn_version", "tgn_last_error", "tgn_launch_count", "tgn_pw_packed_bytes", "tgn_pw_struct_size", "tgn_knn_grid_bytes", "tgn_csr_bytes", "tgn_pt_layer_struct_size", "tgn_pt_layer_sums_struct_size", "tgn_pt_res_apply_struct_size", "tgn_pt_head_struct_size", "tgn_dbscan_bytes", "tgn_knn_f64_bytes", "tgn_kmeans_bytes", "tgn_kdtree_nodes", "tgn_kdtree_bytes", "tgn_kdtree_radius"]
 
 
 class TgnError(RuntimeError):
@@ -188,11 +200,15 @@ def load() -> ctypes.CDLL:
     lib.tgn_pt_layer_struct_size.restype = _i
     lib.tgn_pt_head_struct_size.argtypes = [_i]
     lib.tgn_pt_head_struct_size.restype = _i
+    lib.tgn_pt_layer_sums_struct_size.restype = _i
+    lib.tgn_pt_res_apply_struct_size.restype = _i
     if (lib.tgn_pw_struct_size(0) != ctypes.sizeof(PwLayer) or lib.tgn_pw_struct_size(1) != ctypes.sizeof(PwApply)
             or lib.tgn_pt_layer_struct_size() != ctypes.sizeof(PtLayer)):
         raise TgnError("ctypes mirror of tgn_pw_layer_t / tgn_pw_apply_t / tgn_pt_layer_t is out of date with include/tgn_b200.h")
     if lib.tgn_pt_head_struct_size(0) != ctypes.sizeof(PtUpApply) or lib.tgn_pt_head_struct_size(1) != ctypes.sizeof(HeadClassify):
         raise TgnError("ctypes mirror of tgn_pt_up_apply_t / tgn_head_classify_t is out of date with include/tgn_b200.h")
+    if lib.tgn_pt_res_apply_struct_size() != ctypes.sizeof(PtResApply) or lib.tgn_pt_layer_sums_struct_size() != ctypes.sizeof(PtLayerSums):
+        raise TgnError("ctypes mirror of tgn_pt_res_apply_t / tgn_pt_layer_sums_t is out of date with include/tgn_b200.h")
     _lib = lib
     return lib
 

@@ -57,8 +57,9 @@ def pt_layer_fusable(layer, p, x, o) -> bool:
     return all(_bn_ok(b) for b in (layer.linear_p[1], layer.linear_w[0], layer.linear_w[3]))
 
 
-def pt_layer_forward(layer, pxo) -> torch.Tensor:
-    """blocks.PointTransformerLayer.forward on csrc/pt_layer.cu: (n,3), (n,c), (b) -> (n,c)."""
+def pt_layer_forward(layer, pxo, out_stats: "torch.Tensor | None" = None) -> torch.Tensor:
+    """blocks.PointTransformerLayer.forward on csrc/pt_layer.cu: (n,3), (n,c), (b) -> (n,c).  ``out_stats`` (2c float64, zeroed):
+    the output pass also adds the batch sums {Σ, Σ²} of each output channel to it (``tgn_pt_layer_forward_sums``)."""
     p, x, o = pxo
     x_q, x_k, x_v = layer.linear_q(x), layer.linear_k(x), layer.linear_v(x)         # the model's own nn.Linear GEMMs
     p = p.contiguous()
@@ -88,7 +89,12 @@ def pt_layer_forward(layer, pxo) -> torch.Tensor:
     modes = [_bn_mode(b) for b in (bn_p, bn_a, bn_b)]
     d.bn_mode[0], d.bn_mode[1], d.bn_mode[2] = modes
     d.update_running = 1 if any(m == 1 and b.training and b.running_mean is not None for m, b in zip(modes, (bn_p, bn_a, bn_b))) else 0
-    L.call("tgn_pt_layer_forward", ctypes.byref(d), L.stream_ptr())
+    if out_stats is None:
+        L.call("tgn_pt_layer_forward", ctypes.byref(d), L.stream_ptr())
+    else:
+        ds = L.PtLayerSums()
+        ds.layer, ds.out_stats = d, L.ptr(out_stats)
+        L.call("tgn_pt_layer_forward_sums", ctypes.byref(ds), L.stream_ptr())
     for b in (bn_p, bn_a, bn_b):
         if b.training and b.num_batches_tracked is not None:
             b.num_batches_tracked.add_(1)
@@ -340,3 +346,76 @@ def accelerate_decoder(blocks_module=None, heads_module=None) -> None:
             return mh_orig(self, stage_list)
 
         mhc.forward, mhc._tgn_fused = mh_forward, True
+
+
+# ------------------------------------------------------------------ PointTransformerBlock (blocks.py:114-135)
+
+# The widest block the fused path takes.  Wider blocks (tgnet's first network from 64 channels on) keep the class's previous
+# forward: there linear1 / linear3 on the three-part layer chain cost more device time than the module's cuBLAS Linears save in
+# launches (scripts/pt_block_bench.py, DESIGN §3.7).  The benchmark sets it to compare the widths.
+BLOCK_FUSED_MAX_C = 32
+
+
+def pt_block_fusable(blk, p, x, o) -> bool:
+    """The fused block runs without autograd, on CUDA float32, at widths up to ``BLOCK_FUSED_MAX_C``, with bias-free square
+    linear1 / linear3 (as blocks.py:119, :123 build them; the residual needs in_planes == planes), a transformer layer
+    ``pt_layer_fusable`` takes and BatchNorms torch's own code would not have to take over (``_bn_ok``)."""
+    if not (_enabled and pn2._pw_enabled and _cuda_f32(p, x)):
+        return False
+    lin1, lin3, c = blk.linear1, blk.linear3, x.shape[1]
+    if c > BLOCK_FUSED_MAX_C:
+        return False
+    if lin1.bias is not None or lin3.bias is not None or lin1.weight.dtype != torch.float32 or lin3.weight.dtype != torch.float32:
+        return False
+    if tuple(lin1.weight.shape) != (c, c) or tuple(lin3.weight.shape) != (c, c):
+        return False
+    if not all(type(b) is torch.nn.BatchNorm1d and _bn_ok(b) for b in (blk.bn1, blk.bn2, blk.bn3)):
+        return False
+    return not _needs_grad(blk, p, x) and pt_layer_fusable(blk.transformer2, p, x, o)
+
+
+_blk_chains = weakref.WeakKeyDictionary()         # module -> (linear1's chain, linear3's chain)
+
+
+def pt_block_forward(blk, pxo):
+    """blocks.PointTransformerBlock.forward (:127-135) -> [p, (n, c), o], both BatchNorm modes:
+    * linear1 on the layer chain reading x row-major, bn1 + ReLU written row-major (``tgn_pt_up_apply`` without an addend);
+    * the transformer layer on csrc/pt_layer.cu (the module's own q/k/v Linears), its output pass also forming bn2's batch sums;
+    * linear3 on the chain with bn2 + ReLU applied as it reads the layer's output, and ``tgn_pt_res_apply`` for bn3, the residual
+      add and the ReLU.  Layers whose BatchNorm uses running statistics run promoted accumulation, as the eval-mode chains do.
+    x is only read: the reference's in-place ``+=`` acts on bn3's output."""
+    p, x, o = pxo
+    n, c = x.shape
+    chains = _blk_chains.get(blk)
+    if chains is None:
+        chains = _blk_chains[blk] = (pn2._PwChain(), pn2._PwChain())
+    h = torch.empty((n, c), dtype=torch.float32, device=x.device)
+    chains[0].run([blk.linear1], [blk.bn1], _rows_operand(x, n), n, h, 0, 1, up=(None, None, None), promote=True)
+    bn2 = blk.bn2
+    stats2 = torch.zeros(2 * c, dtype=torch.float64, device=x.device) if pn2._PwChain._bn_mode(bn2) == 1 else None
+    y = pt_layer_forward(blk.transformer2, [p, h, o], stats2)
+    d = _rows_operand(y, n)
+    pn2._PwChain._fill_in_bn(d, bn2, stats2)
+    out = torch.empty((n, c), dtype=torch.float32, device=x.device)
+    chains[1].run([blk.linear3], [blk.bn3], d, n, out, 0, 1, promote=True, residual=x if x.stride(1) == 1 else x.contiguous())
+    if bn2.training and bn2.num_batches_tracked is not None:
+        bn2.num_batches_tracked.add_(1)
+    return [p, out, o]
+
+
+def accelerate_blocks(blocks_module) -> None:
+    """Wrap PointTransformerBlock.forward of an imported reference ``blocks`` module; calls the fused path does not take,
+    autograd included, run the class's previous forward (the reference's, or one whose transformer layer ``accelerate`` wrapped).
+    Idempotent."""
+    blk = blocks_module.PointTransformerBlock
+    if getattr(blk, "_tgn_fused", False):
+        return
+    blk_orig = blk.forward
+
+    def blk_forward(self, pxo):
+        p, x, o = pxo
+        if pt_block_fusable(self, p, x, o):
+            return pt_block_forward(self, pxo)
+        return blk_orig(self, pxo)
+
+    blk.forward, blk._tgn_fused = blk_forward, True

@@ -73,10 +73,15 @@ __device__ __forceinline__ float bn_relu(float x, const BnAffine& a)
 //               output sum (deep levels: a few hundred queries of 128-512 channels, where a single warp walking K neighbours
 //               times c/8 x c products is pure latency).
 // W = 16: two queries per warp, one per half-warp (c = 16 only).
-template <int CPL, int PASS, bool CTAQ, int W = 32>
-__global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_layer_t L)
+// SUMS (pass 3 only): also accumulate fp64 Σ / Σ² per channel of `out` into out_stats, for the BatchNorm that follows the layer
+// in PointTransformerBlock (bn2).  Each element goes into its fp64 sums directly, as in pass 1, so that a channel whose |mean| is
+// far above its std keeps its variance.  The per-lane sums live in shared memory (a row per query slot of a warp, or a slot per
+// channel in the CTA schedule), not in registers: at c = 512 pass 3 already holds 255 registers.
+template <int CPL, int PASS, bool CTAQ, int W = 32, bool SUMS = false>
+__global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_layer_t L, double* out_stats)
 {
     static_assert(W == 32 || (W == 16 && CPL == 1 && !CTAQ), "half-warp queries: c = 16, warp schedule only");
+    static_assert(!SUMS || PASS == 3, "output sums: pass 3 only");
     constexpr int C = W * CPL, CS = C / 8;                     // channels, channels / share_planes (= 8)
     constexpr int QPW = 32 / W;                                // queries per warp
     extern __shared__ __align__(16) unsigned char dyn[];
@@ -95,6 +100,14 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
         ss_a[ch] = scale_shift(L.bn_mode[1], ch, C, L.stats_a, cnt, L.a_gamma, L.a_beta, L.a_eps, L.a_rmean, L.a_rvar);
     if (PASS >= 3) for (int m = tid; m < CS; m += kWarps * 32)
         ss_b[m] = scale_shift(L.bn_mode[2], m, CS, L.stats_b, cnt, L.b_gamma, L.b_beta, L.b_eps, L.b_rmean, L.b_rvar);
+    // SUMS: [slots][2][C] doubles after the logits / partials; slots = kWarps * QPW (warp schedule) or 1 (CTA schedule)
+    constexpr int kSlots = CTAQ ? 1 : kWarps * QPW;
+    double* osum = nullptr;
+    if constexpr (SUMS) {
+        osum = reinterpret_cast<double*>(logits_all + (CTAQ ? static_cast<size_t>(L.K) * CS + kWarps * C
+                                                            : static_cast<size_t>(kWarps) * QPW * L.K * CS));
+        for (int e = tid; e < kSlots * 2 * C; e += kWarps * 32) osum[e] = 0.0;
+    }
     __syncthreads();
     float* logits = CTAQ ? logits_all : logits_all + static_cast<size_t>(warp * QPW + half) * L.K * CS;
     float* out_part = logits_all + static_cast<size_t>(L.K) * CS;           // CTAQ only
@@ -232,6 +245,15 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
             if (valid) {
 #pragma unroll
                 for (int q = 0; q < CPL; ++q) L.out[static_cast<size_t>(i) * C + W * q + sl] = out[q];
+                if constexpr (SUMS) {
+                    double* os = osum + static_cast<size_t>(warp * QPW + half) * 2 * C;
+#pragma unroll
+                    for (int q = 0; q < CPL; ++q) {
+                        const double v = out[q];
+                        os[W * q + sl] += v;
+                        os[C + W * q + sl] = fma(v, v, os[C + W * q + sl]);
+                    }
+                }
             }
             __syncwarp();                                          // the next query's logits overwrite the weights read above
         }
@@ -244,6 +266,11 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) sum += out_part[w * C + ch];
                 L.out[static_cast<size_t>(i) * C + ch] = sum;
+                if constexpr (SUMS) {                                  // channel ch belongs to this thread for every query
+                    const double v = sum;
+                    osum[ch] += v;
+                    osum[C + ch] = fma(v, v, osum[C + ch]);
+                }
             }
             __syncthreads();                                       // logits / partials are reused by the next query
         }
@@ -306,6 +333,14 @@ __global__ void __launch_bounds__(kWarps * 32) pt_layer_kernel(const tgn_pt_laye
             atomicAdd(L.stats_b + which * CS + m, s);
         }
     }
+    if constexpr (SUMS) {
+        __syncthreads();
+        for (int e = tid; e < 2 * C; e += kWarps * 32) {
+            double s = 0.0;
+            for (int w = 0; w < kSlots; ++w) s += osum[w * 2 * C + e];
+            atomicAdd(out_stats + e, s);
+        }
+    }
 }
 
 // torch's training-mode side effect on the three BatchNorms: running = (1 - m) running + m batch (variance unbiased)
@@ -327,19 +362,23 @@ __global__ void pt_update_running_kernel(const tgn_pt_layer_t L)
     }
 }
 
-template <int CPL, int PASS, bool CTAQ, int W = 32>
-int launch_pass_as(const tgn_pt_layer_t& L, cudaStream_t st)
+template <int CPL, int PASS, bool CTAQ, int W = 32, bool SUMS = false>
+int launch_pass_as(const tgn_pt_layer_t& L, cudaStream_t st, double* out_stats = nullptr)
 {
     constexpr int C = W * CPL, CS = C / 8, QPW = 32 / W;
     const size_t head = (C + CS + 4) * sizeof(BnAffine);
     size_t smem = head + static_cast<size_t>(kWarps) * QPW * L.K * CS * sizeof(float);
     smem = std::max(smem, head + static_cast<size_t>(kWarps) * 2 * C * sizeof(double));
     smem = std::max(smem, head + (static_cast<size_t>(L.K) * CS + static_cast<size_t>(kWarps) * C) * sizeof(float));
-    const int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(pt_layer_kernel<CPL, PASS, CTAQ, W>), smem);
+    if (SUMS) {
+        const size_t work = CTAQ ? static_cast<size_t>(L.K) * CS + static_cast<size_t>(kWarps) * C : static_cast<size_t>(kWarps) * QPW * L.K * CS;
+        smem = std::max(smem, head + work * sizeof(float) + static_cast<size_t>(CTAQ ? 1 : kWarps * QPW) * 2 * C * sizeof(double));
+    }
+    const int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(pt_layer_kernel<CPL, PASS, CTAQ, W, SUMS>), smem);
     if (rc != TGN_OK) return rc;
     const int per_cta = CTAQ ? 1 : kWarps * QPW;
     const int grid = std::max(1, std::min((L.n + per_cta - 1) / per_cta, (CTAQ ? 8 : 4) * sm_count()));
-    pt_layer_kernel<CPL, PASS, CTAQ, W><<<grid, kWarps * 32, smem, st>>>(L);
+    pt_layer_kernel<CPL, PASS, CTAQ, W, SUMS><<<grid, kWarps * 32, smem, st>>>(L, out_stats);
     return check_launch("pt_layer_kernel");
 }
 
@@ -347,26 +386,52 @@ int launch_pass_as(const tgn_pt_layer_t& L, cudaStream_t st)
 int g_cta_threshold = 1024;
 
 // c = 16 (W = 16) always runs two queries per warp: the threshold does not apply to it
-template <int CPL, int PASS, int W>
-int launch_pass(const tgn_pt_layer_t& L, cudaStream_t st)
+template <int CPL, int PASS, int W, bool SUMS = false>
+int launch_pass(const tgn_pt_layer_t& L, cudaStream_t st, double* out_stats = nullptr)
 {
-    if constexpr (W == 16) return launch_pass_as<CPL, PASS, false, 16>(L, st);
-    else return L.n < g_cta_threshold ? launch_pass_as<CPL, PASS, true>(L, st) : launch_pass_as<CPL, PASS, false>(L, st);
+    if constexpr (W == 16) return launch_pass_as<CPL, PASS, false, 16, SUMS>(L, st, out_stats);
+    else return L.n < g_cta_threshold ? launch_pass_as<CPL, PASS, true, 32, SUMS>(L, st, out_stats)
+                                      : launch_pass_as<CPL, PASS, false, 32, SUMS>(L, st, out_stats);
 }
 
+// out_stats != NULL: the output pass also accumulates Σ / Σ² of out (tgn_pt_layer_forward_sums)
 template <int CPL, int W = 32>
-int run_layer(const tgn_pt_layer_t& L, cudaStream_t st)
+int run_layer(const tgn_pt_layer_t& L, cudaStream_t st, double* out_stats = nullptr)
 {
     int rc = TGN_OK;
     if (L.bn_mode[0] == 1 && (rc = launch_pass<CPL, 0, W>(L, st)) != TGN_OK) return rc;
     if (L.bn_mode[1] == 1 && (rc = launch_pass<CPL, 1, W>(L, st)) != TGN_OK) return rc;
     if (L.bn_mode[2] == 1 && (rc = launch_pass<CPL, 2, W>(L, st)) != TGN_OK) return rc;
-    if ((rc = launch_pass<CPL, 3, W>(L, st)) != TGN_OK) return rc;
+    rc = out_stats ? launch_pass<CPL, 3, W, true>(L, st, out_stats) : launch_pass<CPL, 3, W>(L, st);
+    if (rc != TGN_OK) return rc;
     if (L.update_running) {
         pt_update_running_kernel<<<(3 + L.c + L.c / 8 + 127) / 128, 128, 0, st>>>(L);
         rc = check_launch("pt_update_running_kernel");
     }
     return rc;
+}
+
+int validate(const tgn_pt_layer_t& L, const char* who)
+{
+    if (L.K < 1 || L.K > 64 || !(L.c == 16 || L.c == 32 || L.c == 64 || L.c == 128 || L.c == 256 || L.c == 512)) {
+        set_error("%s: unsupported shape c=%d K=%d", who, L.c, L.K);
+        return TGN_ERR_INVALID;
+    }
+    if (!L.p || !L.xq || !L.xk || !L.xv || !L.idx || !L.out || !L.p_w0 || !L.p_b0 || !L.p_w1 || !L.p_b1 || !L.a_w || !L.a_b || !L.b_w || !L.b_b ||
+        !L.stats_p || !L.stats_a || !L.stats_b) { set_error("%s: null argument", who); return TGN_ERR_INVALID; }
+    return TGN_OK;
+}
+
+int dispatch(const tgn_pt_layer_t& L, cudaStream_t st, double* out_stats)
+{
+    switch (L.c) {
+        case 16: return run_layer<1, 16>(L, st, out_stats);
+        case 32: return run_layer<1>(L, st, out_stats);
+        case 64: return run_layer<2>(L, st, out_stats);
+        case 128: return run_layer<4>(L, st, out_stats);
+        case 256: return run_layer<8>(L, st, out_stats);
+        default: return run_layer<16>(L, st, out_stats);
+    }
 }
 
 }  // namespace
@@ -389,21 +454,22 @@ int tgn_pt_layer_forward(const tgn_pt_layer_t* layer, void* stream)
     if (!layer) { set_error("pt_layer_forward: null descriptor"); return TGN_ERR_INVALID; }
     const tgn_pt_layer_t& L = *layer;
     if (L.n <= 0) return TGN_OK;
-    if (L.K < 1 || L.K > 64 || !(L.c == 16 || L.c == 32 || L.c == 64 || L.c == 128 || L.c == 256 || L.c == 512)) {
-        set_error("pt_layer_forward: unsupported shape c=%d K=%d", L.c, L.K);
-        return TGN_ERR_INVALID;
-    }
-    if (!L.p || !L.xq || !L.xk || !L.xv || !L.idx || !L.out || !L.p_w0 || !L.p_b0 || !L.p_w1 || !L.p_b1 || !L.a_w || !L.a_b || !L.b_w || !L.b_b ||
-        !L.stats_p || !L.stats_a || !L.stats_b) { set_error("pt_layer_forward: null argument"); return TGN_ERR_INVALID; }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (L.c) {
-        case 16: return run_layer<1, 16>(L, st);
-        case 32: return run_layer<1>(L, st);
-        case 64: return run_layer<2>(L, st);
-        case 128: return run_layer<4>(L, st);
-        case 256: return run_layer<8>(L, st);
-        default: return run_layer<16>(L, st);
-    }
+    const int rc = validate(L, "pt_layer_forward");
+    return rc != TGN_OK ? rc : dispatch(L, static_cast<cudaStream_t>(stream), nullptr);
+}
+
+int tgn_pt_layer_sums_struct_size(void) { return static_cast<int>(sizeof(tgn_pt_layer_sums_t)); }
+
+int tgn_pt_layer_forward_sums(const tgn_pt_layer_sums_t* p, void* stream)
+{
+    using namespace tgn;
+    if (!p) { set_error("pt_layer_forward_sums: null descriptor"); return TGN_ERR_INVALID; }
+    const tgn_pt_layer_t& L = p->layer;
+    if (L.n <= 0) return TGN_OK;
+    int rc = validate(L, "pt_layer_forward_sums");
+    if (rc != TGN_OK) return rc;
+    if (!p->out_stats) { set_error("pt_layer_forward_sums: null out_stats"); return TGN_ERR_INVALID; }
+    return dispatch(L, static_cast<cudaStream_t>(stream), p->out_stats);
 }
 
 }  // extern "C"

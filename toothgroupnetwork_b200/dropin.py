@@ -99,6 +99,19 @@ def accelerate_decoder(blocks_module=None, heads_module=None) -> None:
     blocks_fused.accelerate_decoder(blocks_module, heads_module)
 
 
+def accelerate_transformer_blocks(blocks_module=None) -> None:
+    """Optional: run the no-grad forward of the reference's ``PointTransformerBlock`` (models/modules/cbl_point_transformer/
+    blocks.py:114-135: linear1, its BatchNorms, the transformer layer, linear3 and the residual) on the layer chain,
+    ``csrc/pt_layer.cu``, ``csrc/pt_head.cu`` and ``csrc/pt_block.cu`` through ``toothgroupnetwork_b200.blocks_fused``, at the
+    widths where that is measured to be faster (``blocks_fused.BLOCK_FUSED_MAX_C``); under autograd, at wider blocks and for
+    shapes the kernels do not take, the class's previous forward keeps running.  Imports the module from ``sys.path`` when none
+    is passed."""
+    from . import blocks_fused
+    if blocks_module is None:
+        blocks_module = importlib.import_module("models.modules.cbl_point_transformer.blocks")
+    blocks_fused.accelerate_blocks(blocks_module)
+
+
 def accelerate_inference_pipeline(module=None) -> None:
     """Optional: run the boundary detection and resampling between the two networks of a tgnet inference
     (``InferencePipeLine.get_boundary_sampled_feats``, inference_pipelines/inference_pipeline_tgn.py:289-330: float64 KDTree kNN,

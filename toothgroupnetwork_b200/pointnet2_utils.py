@@ -474,7 +474,7 @@ class _PwChain:
 
     def run(self, convs, bns, first: "L.PwLayer", rows: int, out: torch.Tensor, out_c_offset: int, rows_per_batch_out: int,
             group: int = 0, slopes: Optional[Sequence[float]] = None, relu: bool = True, up: Optional[tuple] = None,
-            promote: bool = False) -> None:
+            promote: bool = False, residual: Optional[torch.Tensor] = None) -> None:
         """``first`` describes the operand source of layer 0 (mode / segments / gather fields filled by the
         caller).  group > 0: the last layer reduces max/min over ``group`` consecutive rows (set abstraction)
         and ``out`` is (B, C_total, rows/group/B...); group == 0: ``out`` receives every row (feature propagation).
@@ -484,7 +484,10 @@ class _PwChain:
         f is None, receives the k = 3 interpolation of f (TransitionUp, blocks.py:110) added to each row.
         ``promote=True``: each layer whose own BatchNorm uses running statistics runs the promoted-accumulation kernel
         (``accum`` = 1: 128-row tiles, the tensor-core accumulator rounded to nearest into an fp32 total every 16 values of K);
-        layers on batch statistics launch exactly as with False."""
+        layers on batch statistics launch exactly as with False.
+        ``residual``: the last BatchNorm goes through ``tgn_pt_res_apply``, ``out`` is (rows, C) row-major and receives
+        relu(bn(y) + residual) with the BatchNorm value rounded first (PointTransformerBlock, blocks.py:132-134); residual is a
+        (rows, C) matrix with unit channel stride."""
         dev = out.device
         n = len(convs)
         couts = [c.weight.shape[0] for c in convs]
@@ -546,7 +549,11 @@ class _PwChain:
         a.update_running = 1 if (mode == 1 and bn.training and bn.running_mean is not None) else 0
         if slopes is not None:
             a.act, a.act_slope = 1, float(slopes[-1])
-        if up is None:
+        if residual is not None:
+            r = L.PtResApply()
+            r.apply, r.identity, r.identity_row_stride = a, L.ptr(residual), residual.stride(0)
+            L.call("tgn_pt_res_apply", ctypes.byref(r), st)
+        elif up is None:
             L.call("tgn_pw_apply", ctypes.byref(a), st)
         else:
             u = L.PtUpApply()
