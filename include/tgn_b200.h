@@ -402,6 +402,8 @@ int tgn_pt_layer_struct_size(void);
 /* layers with fewer queries than this run one CTA per query instead of one warp per query (default 1024); returns the old value.
  * c = 16 layers always run two queries per warp: the threshold does not apply to them. */
 int tgn_pt_layer_set_cta_threshold(int n_queries);
+/* the current threshold, unchanged */
+int tgn_pt_layer_cta_threshold(void);
 /* The same launch with the fp64 batch sums of its output, for the BatchNorm that follows the layer in PointTransformerBlock
  * (blocks.py:131, bn2): out_stats (2c doubles, ACCUMULATED: caller zeroes) = {sum[ch], sumsq[ch]} of out over its n rows, each
  * element added to the fp64 sums as it is written.  `layer` is exactly what tgn_pt_layer_forward takes, and out is bit for bit

@@ -23,6 +23,7 @@ _SIGS = {
     "tgn_knnquery": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_crop_knn": [_i, _i, _i, _i, _vp, _vp, _vp, _i, _vp],
     "tgn_pt_layer_set_cta_threshold": [_i],
+    "tgn_pt_layer_cta_threshold": [],
     "tgn_dbscan": [_i, _vp, ctypes.c_double, _i, _vp, _vp, _vp, _vp, _vp],
     "tgn_knn_f64": [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "tgn_knn_f64_build": [_i, _vp, _vp, _vp],

@@ -12,6 +12,7 @@ of which three are cuDNN BatchNorms over (n, c, K) views -- the largest share of
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import weakref
 
@@ -113,19 +114,39 @@ def transition_down_fusable(td, p, x, o) -> bool:
 
 _td_chains = weakref.WeakKeyDictionary()          # module -> its packed-weight chain; entries go with the module
 
+# True while every offset vector passed to the fused TransitionDown and head-form TransitionUp describes clouds of equal size
+# (a network forward on a (B, C, N) batch, where o0 = N, 2N, ..., BN): their host sizes then come from the tensor shapes, and the
+# new offsets are made on the device, so no offsets are read back and the forward can be captured into a CUDA graph.
+_equal_clouds = False
+
+
+@contextlib.contextmanager
+def equal_clouds():
+    global _equal_clouds
+    old, _equal_clouds = _equal_clouds, True
+    try:
+        yield
+    finally:
+        _equal_clouds = old
+
 
 def transition_down_forward(td, pxo):
     """blocks.TransitionDown.forward (stride != 1, :59-79): FPS, kNN grouping [xyz_rel | feats], Linear + BatchNorm + ReLU, max over K
     -- a one-layer set abstraction over kNN neighbourhoods -- on the tensor-core layer chain (batch statistics included)."""
     p, x, o = pxo
-    host_o = o.cpu().tolist()                                    # the reference reads o[i].item() here too (:64-67)
-    n_o, count, prev = [], 0, 0
-    for e in host_o:
-        count += (e - prev) // td.stride
-        n_o.append(count)
-        prev = e
-    n_o = torch.tensor(n_o, dtype=torch.int32, device=o.device)
-    sizes = [host_o[0]] + [host_o[i] - host_o[i - 1] for i in range(1, len(host_o))]
+    if _equal_clouds:
+        b, size = o.shape[0], p.shape[0] // o.shape[0]
+        sizes, count = [size] * b, b * (size // td.stride)
+        n_o = torch.arange(1, b + 1, dtype=torch.int32, device=o.device).mul_(size // td.stride)
+    else:
+        host_o = o.cpu().tolist()                                # the reference reads o[i].item() here too (:64-67)
+        n_o, count, prev = [], 0, 0
+        for e in host_o:
+            count += (e - prev) // td.stride
+            n_o.append(count)
+            prev = e
+        n_o = torch.tensor(n_o, dtype=torch.int32, device=o.device)
+        sizes = [host_o[0]] + [host_o[i] - host_o[i - 1] for i in range(1, len(host_o))]
     p = p.contiguous()
     idx = pointops.fps_packed(p, o, n_o, max(sizes), count)
     n_p = p[idx.long(), :]
@@ -160,7 +181,7 @@ def accelerate(blocks_module) -> None:
         return td_orig(self, pxo)
 
     ptl.forward, tdc.forward = ptl_forward, td_forward
-    ptl._tgn_fused = True
+    ptl._tgn_fused = tdc._tgn_fused = True
 
 
 # ------------------------------------------------------------------ decoder and heads (blocks.py:82-111, heads.py:13-61)
@@ -197,6 +218,8 @@ def transition_up_fusable(tu, pxo1, pxo2=None) -> bool:
     if pxo2 is None:
         if not _cuda_f32(x1) or _needs_grad(tu, x1) or not transition_up_structure_ok(tu, True, x1.shape[1]):
             return False
+        if _equal_clouds:
+            return x1.shape[0] % o1.shape[0] == 0
         ends = o1.cpu().tolist()
         return ends[-1] == x1.shape[0] and all(e == (b + 1) * ends[0] for b, e in enumerate(ends))
     p2, x2, o2 = pxo2

@@ -448,6 +448,8 @@ int tgn_pt_layer_set_cta_threshold(int n_queries)
     return old;
 }
 
+int tgn_pt_layer_cta_threshold(void) { return tgn::g_cta_threshold; }
+
 int tgn_pt_layer_forward(const tgn_pt_layer_t* layer, void* stream)
 {
     using namespace tgn;

@@ -112,6 +112,20 @@ def accelerate_transformer_blocks(blocks_module=None) -> None:
     blocks_fused.accelerate_blocks(blocks_module)
 
 
+def accelerate_graphs(module=None) -> None:
+    """Optional: replay the no-grad forward of the reference's point-transformer network (``PointTransformerSeg.forward``,
+    models/modules/cbl_point_transformer/cbl_point_transformer_module.py:93-216) as a CUDA graph through
+    ``toothgroupnetwork_b200.graphs``: per module and input shape, the first call runs eagerly, the second captures and replays,
+    later calls replay.  Only calls whose TransitionDowns, TransitionUps and heads all take the fused paths of
+    ``accelerate_blocks`` and ``accelerate_decoder`` are graphed; every other call (autograd, targets, other configurations) runs
+    the class's previous forward.  ``graphs.release_graphs()`` frees the graphs.  Imports the module from ``sys.path`` when none
+    is passed."""
+    from . import graphs
+    if module is None:
+        module = importlib.import_module("models.modules.cbl_point_transformer.cbl_point_transformer_module")
+    graphs.accelerate(module)
+
+
 def accelerate_inference_pipeline(module=None) -> None:
     """Optional: run the boundary detection and resampling between the two networks of a tgnet inference
     (``InferencePipeLine.get_boundary_sampled_feats``, inference_pipelines/inference_pipeline_tgn.py:289-330: float64 KDTree kNN,
